@@ -1,5 +1,5 @@
 """The hot-path census of one `swap()` (SURVEY Appendix B) on the STOCK reference modules -- the comparator arms of
-bench.py.  Same call list as bench.py's own step, but through the unmodified classes of the staged checkout:
+bench.py.  Same call list as bench.py's own step, but through the unmodified classes of the built reference:
 `models.stylegan2.model.Generator` (F.conv2d(groups=B) / conv_transpose2d through cuDNN + the two JIT kernels,
 models/stylegan2/model.py:238-279), `Encoder4Editing`, `fs_encoder_v2`, `FeatureEncoderMult`, `FeatureiResnet`, `BiSeNet`.
 

@@ -1,6 +1,6 @@
-"""Run the UNMODIFIED reference checkout (staged by tools/stage_reference.sh into baseline/_ref/HairFastGAN) in this
-image: import-time stand-ins for the packages the image lacks (SURVEY Appendix D: clip, dlib, face_alignment, lpips,
-matplotlib, gdown, addict, torchmetrics -> baseline/stubs/), the prebuilt JIT-extension cache, the working directory
+"""Run the UNMODIFIED reference (built by oracle/build_ref.py into oracle/_ref: sourceless bytecode of the checkout plus
+its two prebuilt JIT extensions) in this image: import-time stand-ins for the packages the image lacks (SURVEY Appendix D: clip, dlib, face_alignment, lpips,
+matplotlib, gdown, addict, torchmetrics -> baseline/stubs/), the prebuilt JIT extensions, the working directory
 the reference's relative paths assume (`pretrained_models/...`, `models/sean_codes/styles_test/...`), and -- optionally
 -- this package's overlay (hairfastgan_b200.install) on top.
 
@@ -19,32 +19,42 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
 STUBS = os.path.join(HERE, "stubs")
-REF_DIR = os.path.join(HERE, "_ref")
+REF_DIR = os.path.join(REPO, "oracle", "_ref")
 REF_ROOT = os.path.join(REF_DIR, "HairFastGAN")
 EXT_DIR = os.path.join(REF_DIR, "ext")
 
 
 def available() -> bool:
-    return os.path.isfile(os.path.join(REF_ROOT, "hair_swap.py"))
+    return os.path.isfile(os.path.join(REF_ROOT, "hair_swap.pyc"))
 
 
 def ref_root() -> str:
     if not available():
-        raise RuntimeError(f"reference not staged at {REF_ROOT}: run tools/stage_reference.sh (needs /root/reference)")
+        raise RuntimeError(f"reference not built at {REF_ROOT}: run oracle/build_ref.py (needs a reference checkout)")
     return REF_ROOT
+
+
+def _prebuilt_extension(name, sources=None, *args, **kwargs):
+    """Stands in for torch.utils.cpp_extension.load in the reference's op/ modules: imports the extension
+    oracle/build_ref.py built with that same builder (the sources it would hash are not part of the build)."""
+    import importlib.util
+    path = os.path.join(EXT_DIR, name, name + ".so")
+    spec = importlib.util.spec_from_file_location(name, path)
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
 
 
 def activate(overlay: bool, skip_fse_reconstruction: bool = False, chdir: bool = True, workdir: str | None = None,
              **install_kwargs) -> str:
-    """Put the staged reference (and the stand-ins) on sys.path; returns the reference root.
+    """Put the built reference (and the stand-ins) on sys.path; returns the reference root.
 
     workdir: directory holding `pretrained_models/` (see baseline/synth_checkpoints.py).  The reference resolves every
     checkpoint and SEAN's style codes relative to the cwd, so `workdir` gets symlinks to the reference's top-level
     entries and becomes the cwd."""
     root = ref_root()
-    os.environ.setdefault("TORCH_EXTENSIONS_DIR", EXT_DIR)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")      # same nvcc line here (no GPU) and on the B200 box
-    os.environ.setdefault("MAX_JOBS", "8")
+    import torch.utils.cpp_extension
+    torch.utils.cpp_extension.load = _prebuilt_extension
     for p in (STUBS, root, REPO):
         if p in sys.path:
             sys.path.remove(p)

@@ -2,7 +2,7 @@
 
     python baseline/run_swap.py --mode reference|overlay|overlay_fast --work DIR --out result.pt [--reps N]
 
-* reference     the staged, unmodified checkout: cuDNN grouped convolutions + its two JIT kernels, fp32/TF32
+* reference     the unmodified reference (oracle/_ref): cuDNN grouped convolutions + its two JIT kernels, fp32/TF32
 * overlay       the same checkout with hairfastgan_b200.install() active (this package's modules under its names)
 * overlay_fast  overlay + install(skip_fse_reconstruction=True) (hairfastgan_b200/fse_fast.py)
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- hair-swap hot-path throughput on B200 (contract: see DESIGN.md "Measurement").
+"""bench.py -- hair-swap hot-path throughput on H100 (contract: see DESIGN.md "Measurement").
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--triples T]
 
@@ -44,7 +44,8 @@ GFLOP_PP_PER_TRIPLE = 2 * GFLOP_PP_ENC_IMG + GFLOP_PP_RES
 GFLOP_SEG_512 = 27.5                                      # BiSeNet (ResNet-18 context path + heads) on one 512^2 image
 GFLOP_SEG_PER_TRIPLE = 3 * GFLOP_SEG_512 + 2 * 4 * GFLOP_SEG_512      # 3 calls at 512^2, 2 at 1024^2 (SURVEY 8f-3)
 GFLOP_PER_TRIPLE = GFLOP_GEN_PER_TRIPLE + GFLOP_ENC_PER_TRIPLE + GFLOP_PP_PER_TRIPLE + GFLOP_SEG_PER_TRIPLE   # = 3063.8
-ROOFLINE_US_PER_IMG = 142.5                               # SURVEY Appendix A, sum of per-layer maxima
+REF_GPU_MAX_T = 16                                        # largest step of the reference_gpu leg (see there)
+ROOFLINE_US_PER_IMG = 244.1                               # SURVEY Appendix A (H100 SXM data sheet), sum of per-layer maxima
 
 
 def peaks():
@@ -53,11 +54,11 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d["bf16_tflops_sustained"],
                 "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "src": "fallback"}
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
 
     def __init__(self, index: int):
         self.index, self.rows, self.proc = index, [], None
@@ -183,36 +184,40 @@ def run_ours(args, rank, world, local_rank):
     host_out = torch.empty(T, 3, 1024, 1024).pin_memory()
     launches = [0]
 
-    def compute(inp, skip_fse_recon=False, full_seg=False):
-        """The hot path of T triples through the public module API (what swap()'s stages call)."""
+    def compute(inp, skip_fse_recon=False, full_seg=False, keep=None):
+        """The hot path of T triples through the public module API (what swap()'s stages call).  `keep`: a dict that
+        receives every stage's output by name (references only, nothing is copied)."""
         img, lats, lins, calls = inp["img"], inp["lat"], inp["lin"], inp["calls"]
+        kept = keep if keep is not None else {}
         n0 = lib.hf_total_launch_count() + graphs.stats()["replayed_kernels"]   # eager launches + kernels inside replayed graphs
-        for net, x in ((e4e, img[0]), (e4e, img[1]), (fse, img[2])):   # Embedding.py:71,74 / :51
-            net(x)
+        for name, net, x in (("e4e_a", e4e, img[0]), ("e4e_b", e4e, img[1]), ("fse", fse, img[2])):   # Embedding.py:71,74 / :51
+            kept[name] = net(x)
         final = None
         for i, (s, e, b, r) in enumerate(calls):
             if i == 0 and skip_fse_recon:              # opt-in 8f-2 fast path: same RNG draws, no reconstruction
                 gen.consume_noise(b)
                 continue
             out = gen([lats[i]], input_is_latent=True, start_layer=s, end_layer=e, layer_in=lins[i])   # random noise
+            kept[f"generator_{i}"] = out
             if i == len(calls) - 1:
                 final = out[0]
-        _, (f_face,) = pp_enc(img[3])                  # PostProcessModel.forward, models/Encoders.py:120-139
-        _, (f_hair,) = pp_enc(img[4])
-        pp_res(torch.cat((f_face, f_hair), dim=1))
+        kept["pp_enc_face"] = (_, (f_face,)) = pp_enc(img[3])        # PostProcessModel.forward, models/Encoders.py:120-139
+        kept["pp_enc_hair"] = (_, (f_hair,)) = pp_enc(img[4])
+        kept["pp_res"] = pp_res(torch.cat((f_face, f_hair), dim=1))
         # get_segmentation x3 at 512^2 and twice at 1024^2 (models/Net.py:108-115).  Under install()'s defaults the
         # reference's FaceParsing_tensor.parsing_img runs the label-only path (parsing_fast.py: bit-identical labels,
         # aux heads + full-resolution logits not materialised); `full_seg=True` = the module's three-logit forward
         parse = seg if full_seg else seg.parse_labels
-        parse(img[5])
-        parse(img[6]); parse(img[6])
+        kept["seg_512"] = parse(img[5])
+        kept["seg_1024"] = parse(img[6]); parse(img[6])
         launches[0] += lib.hf_total_launch_count() + graphs.stats()["replayed_kernels"] - n0
         return final
 
-    def step():
-        return compute(devin)
+    def step(keep=None):
+        return compute(devin, keep=keep)
 
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 50 MB L2
+    dumped = {}                                                        # outputs of the last timed step (--dump-outputs)
 
     def timed(steps: int, warmup: int):
         for _ in range(warmup):
@@ -223,11 +228,14 @@ def run_ours(args, rank, world, local_rank):
         torch.cuda.synchronize()
         launches[0] = 0
         total_ms = 0.0
-        for _ in range(steps):
+        for k in range(steps):
+            last = k == steps - 1 and args.dump_outputs
+            if last:
+                torch.manual_seed(3407)                                # the dumped step's noise draws do not depend on K
             flush.fill_(1)                                             # L2 flush between timed iterations
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            step()
+            step(dumped if last else None)
             e1.record()
             e1.synchronize()
             total_ms += e0.elapsed_time(e1)
@@ -306,6 +314,9 @@ def run_ours(args, rank, world, local_rank):
     torch.cuda.synchronize()
     first = sampler.mark()
     ms, n_launch = timed(args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(dumped, args.dump_outputs)
+        dumped.clear()
     ms_e2e = timed_e2e(args.steps, max(3, args.warmup // 2))
     clocks = sampler.stop(first) if rank == 0 else None
 
@@ -372,7 +383,7 @@ def run_ours(args, rank, world, local_rank):
         lat4 = torch.randn(4, 18, 512, device=dev)
         us_img = avg_ms(lambda: gen([lat4], input_is_latent=True)) / 4 * 1e3
         extra["generator_b4"] = {"img_per_s": round(1e6 / us_img, 1), "us_per_img": round(us_img, 1),
-                                 "frac_of_roofline_142.5us": round(ROOFLINE_US_PER_IMG / us_img, 4),
+                                 f"frac_of_roofline_{ROOFLINE_US_PER_IMG}us": round(ROOFLINE_US_PER_IMG / us_img, 4),
                                  "tflops_algorithmic": round(GFLOP_FULL / us_img * 1e3, 1)}
         # configs[3]: e4e + FSE inversion, 256^2, batch 32
         x32 = torch.rand(32, 3, 256, 256, device=dev) * 2 - 1
@@ -438,7 +449,7 @@ def _json_tail(stdout: str):
 
 def comparator_legs(args):
     """Side measurements that need OTHER processes (the GPU is free: our own run has finished): the stock reference on
-    the same B200 (`reference_gpu`), the full HairFast.swap() under the overlay vs the stock one (`full_swap`), and our
+    the same GPU (`reference_gpu`), the full HairFast.swap() under the overlay vs the stock one (`full_swap`), and our
     own step with every network in bf16 / fp16 (`value_by_dtype`).  Each is a bounded child run; a failure is reported
     in the line, never hidden."""
     from baseline import refenv
@@ -466,15 +477,17 @@ def comparator_legs(args):
     out["value_by_dtype"] = {"unit": "triples/s", "note": "every network in that operand type (HAIRFAST_DTYPE=...)",
                              **by_dtype}
     if not refenv.available():
-        out["reference_gpu"] = {"unavailable": "reference checkout not staged (tools/stage_reference.sh)"}
-        out["full_swap"] = {"unavailable": "reference checkout not staged (tools/stage_reference.sh)"}
+        out["reference_gpu"] = {"unavailable": "reference not built (oracle/build_ref.py)"}
+        out["full_swap"] = {"unavailable": "reference not built (oracle/build_ref.py)"}
         return out
     census_py = os.path.join(ROOT, "baseline", "ref_census.py")
     ref = {}
     # T = 1 (latency) and the largest batching the stock modules survive: at T = 32 (B = 96 in the full forwards) the
     # reference dies with a CUDA error inside its own kernels (index overflow past 2^31 elements), so the sweep walks
     # down from our T until a census completes
-    t_try = [1] + [t for t in (args.triples, 16, 8) if t > 1]
+    # the stock reference stops with a CUDA error inside its own code at 32 triples per step (3T = 96 images per
+    # generator call), so this leg does not go past REF_GPU_MAX_T
+    t_try = [1] + [t for t in (min(args.triples, REF_GPU_MAX_T), 8) if t > 1]
     done_big = False
     for T in dict.fromkeys(t_try):
         if T > 1 and done_big:
@@ -490,7 +503,7 @@ def comparator_legs(args):
             msg = str(ex)
             ref[f"T{T}"] = {"error": ("CUDA error inside the stock reference at this batch: " if "CUDA" in msg else "")
                             + msg.strip().splitlines()[-1][-160:] if msg.strip() else "failed"}
-    ref["what"] = ("the SAME census on the stock reference modules on this B200: F.conv2d(groups=B)/conv_transpose2d "
+    ref["what"] = ("the SAME census on the stock reference modules on this GPU: F.conv2d(groups=B)/conv_transpose2d "
                    "through cuDNN + its two JIT kernels (models/stylegan2/model.py:238-279), baseline/ref_census.py")
     out["reference_gpu"] = ref
     swap = {}
@@ -519,6 +532,44 @@ def comparator_legs(args):
                     "stack + BiSeNet (forward hooks, CUDA events); out of scope = SEAN, CLIP stand-in, mask nets, glue")
     out["full_swap"] = swap
     return out
+
+
+DUMP_BYTES = 64 << 20          # --dump-outputs: at most this much in all
+DUMP_FINAL_ELEMS = 4 << 20     # elements kept of the final images; every other array keeps at most DUMP_ELEMS
+DUMP_ELEMS = 1 << 19
+
+
+def dump_outputs(outputs, out_dir):
+    """Write each output array of one step as out_dir/<name>.npy (float32).  An array larger than its share keeps a
+    fixed sample: the elements at sorted flat indices drawn from a generator seeded by the array's size, so two builds
+    of the project sample the same positions."""
+    import numpy as np
+    import torch
+    flat = {}
+
+    def add(name, v):
+        if torch.is_tensor(v):
+            flat[name] = v
+        elif isinstance(v, (tuple, list)):
+            for i, x in enumerate(v):
+                add(f"{name}.{i}", x)
+
+    for name, v in outputs.items():
+        add(name, v)
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, t in flat.items():
+        cap = DUMP_FINAL_ELEMS if name == "generator_7.0" else DUMP_ELEMS
+        t = t.detach().reshape(-1)
+        if t.numel() > cap:
+            g = torch.Generator(device="cpu").manual_seed(t.numel())
+            idx = torch.randint(t.numel(), (cap,), generator=g).sort().values
+            t = t[idx.to(t.device)]
+        a = t.float().cpu().numpy().astype(np.float32)
+        total += a.nbytes
+        if total > DUMP_BYTES:
+            raise RuntimeError(f"--dump-outputs would exceed {DUMP_BYTES >> 20} MB at {name}")
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def time_dominant_kernel(gen, dev, B=4):
@@ -571,9 +622,8 @@ CPU_SAMPLE = ("every distinct call of the SURVEY App. B census once at B=1 (gene
 
 
 def cpu_threads():
-    """Physical host cores, stated.  torchrun exports OMP_NUM_THREADS=1 to its workers (round 1: 64 threads at N=1, one
-    thread under torchrun -> a 4.5x swing of the denominator), and os.cpu_count() counts hyper-threads (128 on the B200
-    hosts: measured 40x SLOWER than 64 threads on these B=1 convolutions), so neither is inherited silently."""
+    """Physical host cores, stated.  torchrun exports OMP_NUM_THREADS=1 to its workers, and os.cpu_count() counts
+    hyper-threads (oversubscribing the B=1 convolutions slows them down), so neither is inherited silently."""
     try:
         import psutil
         n = psutil.cpu_count(logical=False)
@@ -588,7 +638,7 @@ def cpu_threads():
 
 
 def cpu_census_reference(steps: int, warmup: int):
-    """The STOCK reference modules (staged checkout, baseline/_ref) on the host cores: baseline/ref_census.py."""
+    """The STOCK reference modules (oracle/_ref, built by oracle/build_ref.py) on the host cores: baseline/ref_census.py."""
     env = dict(os.environ)
     env.pop("OMP_NUM_THREADS", None)
     cmd = [sys.executable, os.path.join(ROOT, "baseline", "ref_census.py"), "--device", "cpu", "--steps", str(steps),
@@ -601,7 +651,7 @@ def cpu_census_reference(steps: int, warmup: int):
 
 
 def cpu_census_port(steps: int, warmup: int):
-    """Same census on the oracle port (used only when the reference checkout is not staged)."""
+    """Same census on the oracle port (used only when the reference is not built)."""
     import torch
     from oracle import stylegan2_oracle as O
     from oracle import encoders_oracle as EO
@@ -698,6 +748,8 @@ def main():
     ap.add_argument("--triples", type=int, default=32, help="independent triples batched per step and GPU")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the per-network / per-operator side measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, sampled, <= 64 MB)")
     ap.add_argument("--profile-step", action="store_true", help="run one step between cudaProfilerStart/Stop, no JSON")
     ap.add_argument("--no-comparators", action="store_true",
                     help="skip the child-process legs (reference_gpu, full_swap, value_by_dtype)")

@@ -1,4 +1,4 @@
-"""ctypes binding of libhairfast_sm100.so (include/hairfast_b200.h).
+"""ctypes binding of libhairfast_sm90.so (include/hairfast_b200.h).
 
 There is NO fallback: if the shared library is missing the import fails loudly, and every call
 checks the status code and raises RuntimeError with hf_last_error() -- the same error type the
@@ -10,7 +10,7 @@ import ctypes as C
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(HERE, "csrc", "libhairfast_sm100.so")
+LIB_PATH = os.path.join(HERE, "csrc", "libhairfast_sm90.so")
 
 HF_BF16, HF_F16 = 0, 1
 HF_MAX_STYLED, HF_MAX_TORGB = 17, 9

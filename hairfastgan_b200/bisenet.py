@@ -1,4 +1,4 @@
-"""BiSeNet face parsing (SURVEY 8f-3) on the tcgen05 convolution kernels.
+"""BiSeNet face parsing (SURVEY 8f-3) on the wgmma convolution kernels.
 
 Drop-in counterpart of ``models/CtrlHair/external_code/face_parsing/model.py`` + ``resnet.py`` (the network
 ``FaceParsing`` builds, my_parsing_util.py:42,77, and ``get_segmentation`` runs five times per swap, models/Net.py:108-115):

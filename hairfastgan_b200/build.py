@@ -1,4 +1,4 @@
-"""Build libhairfast_sm100.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libhairfast_sm90.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m hairfastgan_b200.build [--force]
 """
@@ -10,7 +10,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-LIB = os.path.join(CSRC, "libhairfast_sm100.so")
+LIB = os.path.join(CSRC, "libhairfast_sm90.so")
 SOURCES = ["hf_api.cu", "hf_ops.cu", "hf_conv_tc.cu", "hf_generator.cu", "hf_enc_ops.cu", "hf_enc_api.cu",
            "hf_seg_ops.cu", "hf_glue_ops.cu"]
 HEADERS = ["hf_common.cuh", "hf_kernels.cuh", os.path.join("..", "..", "include", "hairfast_b200.h")]
@@ -35,7 +35,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not needs_build():
         return LIB
     objs = []
-    flags = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    flags = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
              "-Xcompiler", "-fPIC", "--use_fast_math=false"]
     flags = [f for f in flags if f != "--use_fast_math=false"]
     if verbose:
@@ -52,7 +52,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError("nvcc failed: %s\n%s" % (" ".join(cmd), out))
         if verbose and out:
             print(out)
-    cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed: %s\n%s" % (" ".join(cmd), r.stdout))

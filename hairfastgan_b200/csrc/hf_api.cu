@@ -28,10 +28,10 @@ int num_sms() {
   static int sms[64] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return 148;
+  if (dev < 0 || dev >= 64) return 132;
   if (!sms[dev]) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     sms[dev] = n;
   }
   return sms[dev];
@@ -116,7 +116,7 @@ using namespace hf;
 
 extern "C" {
 
-int hf_version(void) { return 100; }
+int hf_version(void) { return 90; }
 const char* hf_last_error(void) { return g_err; }
 int hf_last_launch_count(void) { return g_launches; }
 long long hf_total_launch_count(void) { return hf::total_launch_count(); }
@@ -129,8 +129,8 @@ int hf_set_device(int device) {
   int major = 0, minor = 0;
   HF_CUDA_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
   HF_CUDA_OK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-  if (major != 10) {
-    set_error("device %d is sm_%d%d; libhairfast_sm100 only contains sm_100a code and has no fallback", device,
+  if (major != 9) {
+    set_error("device %d is sm_%d%d; libhairfast_sm90 only contains sm_90a code and has no fallback", device,
               major, minor);
     return HF_ERR_UNSUPPORTED;
   }

@@ -1,5 +1,5 @@
-// Common helpers for the sm_100a kernels: error plumbing, PTX wrappers for
-// mbarrier / TMA / tcgen05 (inline PTX only -- no CUTLASS dependency).
+// Common helpers for the sm_90a kernels: error plumbing, PTX wrappers for
+// mbarrier / TMA / wgmma (inline PTX only -- no CUTLASS dependency).
 #pragma once
 #include <cuda.h>          // CUtensorMap (types only; the encode entry point is fetched at run time)
 #include <cuda_runtime.h>
@@ -120,6 +120,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// The same bound without the printf: for waits between wgmma issue and wgmma.wait_group, where a function call
+// would make ptxas serialise the MMA pipeline.
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > 4000000000LL) __trap();
+  }
+}
+
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -142,221 +152,135 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// --- tcgen05 / TMEM ---------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {   // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {     // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; one thread issues for the CTA.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// The MMA main loops run inside ONE elected lane (`if (elect_one()) { ... }`, CUTLASS style): issuing under
-// `if (lane == 0)` made ptxas wrap every UTCHMMA in an R2UR waterfall loop (~450 issue cycles per conv tap, measured).
-// Single-thread forms, to be used inside `if (elect_one()) { ... }` (CUTLASS style: the whole MMA main loop
-// runs in ONE elected lane, so ptxas needs neither waterfall loops nor per-instruction elect/vote).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-template <int NK>
-__device__ __forceinline__ void umma_tap(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                         uint32_t idesc, uint32_t acc_first) {
-  static_assert(NK == 2 || NK == 4, "NK must be 2 or 4");
-  if (NK == 4) {
-    asm volatile(
-        "{\n\t.reg .pred p, t;\n\t.reg .b64 da, db;\n\t.reg .b32 al, bl;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "setp.eq.b32 t, 0, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-        "add.u32 al, %1, 2;\n\tadd.u32 bl, %3, 2;\n\tmov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n\t"
-        "add.u32 al, %1, 4;\n\tadd.u32 bl, %3, 4;\n\tmov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n\t"
-        "add.u32 al, %1, 6;\n\tadd.u32 bl, %3, 6;\n\tmov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n\t}"
-        ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(acc_first)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p, t;\n\t.reg .b64 da, db;\n\t.reg .b32 al, bl;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "setp.eq.b32 t, 0, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-        "add.u32 al, %1, 2;\n\tadd.u32 bl, %3, 2;\n\tmov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n\t}"
-        ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(acc_first)
-        : "memory");
-  }
-}
-// one MMA, descriptors given as (lo, hi) words; single issuing thread
-__device__ __forceinline__ void umma_one(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 
-// ----------------------------------------------------------------------------------------
-// CTA-pair (cta_group::2) forms.  A shared::cta address is a valid shared::cluster address of the executing
-// CTA; clearing bit 24 addresses the same offset in the even (leader) CTA of the pair (CUTLASS
-// Sm100MmaPeerBitMask).
-// ----------------------------------------------------------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {     // arrive on the leader CTA's copy of `bar`
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-__device__ __forceinline__ void tma2_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* leader_bar, int c0,
-                                             int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(leader_bar) & kPeerBitMask),
-      "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* leader_bar, int c0,
-                                             int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(leader_bar) & kPeerBitMask),
-      "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_dst, uint32_t ncols) {   // whole warp, both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// commit of the leader's MMAs, arriving on the barrier at the same smem offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit2(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-      : "memory");
-}
-// four K=16 MMAs of one conv tap, M=256 across the CTA pair (single issuing thread of the leader CTA)
-__device__ __forceinline__ void umma_tap2_x4(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                             uint32_t b_hi, uint32_t idesc, uint32_t acc_first) {
-  asm volatile(
-      "{\n\t.reg .pred p, t;\n\t.reg .b64 da, db;\n\t.reg .b32 al, bl;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "setp.eq.b32 t, 0, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, p;\n\t"
-      "add.u32 al, %1, 2;\n\tadd.u32 bl, %3, 2;\n\tmov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, t;\n\t"
-      "add.u32 al, %1, 4;\n\tadd.u32 bl, %3, 4;\n\tmov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, t;\n\t"
-      "add.u32 al, %1, 6;\n\tadd.u32 bl, %3, 6;\n\tmov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, t;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-
-__device__ __forceinline__ uint32_t kmajor_desc_lo(uint32_t smem_addr) {
-  return ((smem_addr & 0x3FFFF) >> 4) | (1u << 16);
-}
-// High 32 bits of a K-major descriptor (SBO, version, layout); the low word is (addr >> 4) | LBO.
-__device__ __forceinline__ uint32_t kmajor_desc_hi(uint32_t sbo_bytes, uint32_t layout_type) {
-  return ((sbo_bytes >> 4) & 0x3FFF) | (1u << 14) | ((layout_type & 7) << 29);
-}
-__device__ __forceinline__ uint64_t kmajor_desc(uint32_t hi, uint32_t smem_addr) {
-  return ((uint64_t)hi << 32) | (uint64_t)(((smem_addr & 0x3FFFF) >> 4) | (1u << 16));
-}
-
-// 32 lanes x 32 consecutive fp32 columns; thread i of the warp gets lane (base_lane + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32_x8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// K-major shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [49,52) base_offset | [61,64) layout
-// For the swizzled K-major canonical layouts rows are `swizzle_bytes` wide, an 8-row group is
-// 8*swizzle_bytes contiguous, and SBO is the distance between 8-row groups.
-__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t layout_type) {
+// --- wgmma (Hopper warpgroup MMA, accumulators in registers) ---------------------------------
+// Shared-memory matrix descriptor (PTX "matrix descriptor format" for wgmma):
+//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base_offset | [62,64) swizzle mode
+// For the swizzled K-major layouts rows are `swizzle_bytes` wide, an 8-row group is 8*swizzle_bytes contiguous,
+// SBO is the distance between 8-row groups and LBO is unused.  Advancing K by 16 elements inside the swizzle
+// atom adds 32 bytes (2 descriptor units) to the start address.
+constexpr uint32_t GMMA_LAYOUT_SW128 = 1;
+constexpr uint32_t GMMA_LAYOUT_SW64 = 2;
+__device__ __forceinline__ uint64_t make_gmma_desc(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t layout_type) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;                          // LBO (ignored for swizzled K-major)
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;                          // descriptor version 1 (Blackwell)
-  d |= (uint64_t)(layout_type & 7) << 61;
+  d |= (uint64_t)(layout_type & 3) << 62;
   return d;
 }
-constexpr uint32_t UMMA_LAYOUT_SW128 = 2;
-constexpr uint32_t UMMA_LAYOUT_SW64 = 4;
-
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): fp32 accumulate, K-major A and B.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int dtype, int m, int n) {
-  return (1u << 4)                                   // c_format = F32
-         | ((dtype == HF_BF16 ? 1u : 0u) << 7)       // a_format
-         | ((dtype == HF_BF16 ? 1u : 0u) << 10)      // b_format
-         | (0u << 15) | (0u << 16)                   // a_major, b_major = K
-         | ((uint32_t)(n >> 3) << 17)                // n_dim
-         | ((uint32_t)(m >> 4) << 24);               // m_dim
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// Keeps the accumulator registers live across the asynchronous MMAs (the compiler must not move accesses to them
+// across wgmma.fence / wait_group).
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (fp32, registers of the warpgroup) += A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory.
+template <int N, int DT> struct Wgmma;
+template <> struct Wgmma<32, HF_BF16> {
+  static __device__ __forceinline__ void mma(float (&d)[16], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db));
+  }
+};
+template <> struct Wgmma<32, HF_F16> {
+  static __device__ __forceinline__ void mma(float (&d)[16], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db));
+  }
+};
+template <> struct Wgmma<64, HF_BF16> {
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db));
+  }
+};
+template <> struct Wgmma<64, HF_F16> {
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db));
+  }
+};
+template <> struct Wgmma<128, HF_BF16> {
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db));
+  }
+};
+template <> struct Wgmma<128, HF_F16> {
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db));
+  }
+};
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

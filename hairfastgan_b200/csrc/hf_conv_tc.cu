@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM convolution for sm_100a: the ModulatedConv2d / StyledConv hot loop.
+// wgmma implicit-GEMM convolution for sm_90a: the ModulatedConv2d / StyledConv hot loop.
 //
 //   y[b,o,p] = act( d[b,o] * sum_{tap,c} W~[o,tap,c] * xh[b, p+tap, c]  + nw*noise[b,p] + bias[o] )
 //
@@ -7,32 +7,24 @@
 // 16-bit NHWC activation `xh` by the producer of that tensor, the demodulation d[b,o] is applied to
 // the fp32 accumulator in the epilogue).  The upsampling conv (conv_transpose2d stride 2 + 4x4 blur,
 // model.py:252-263) runs as four 3x3 correlations, one per output parity, stacked along GEMM-N
-// (Appendix C-2), so the same kernels serve both.
+// (Appendix C-2), so the same kernel serves both.
 //
-// GEMM view per tile:  D[128 pixels, n_tile] += A[128 pixels, 64 ch] * B[n_tile, 64 ch]^T over taps x
-// channel chunks; operands in swizzled K-major shared memory, tcgen05.mma kind::f16 with fp32
-// accumulators in TMEM, persistent CTAs with a static schedule, two accumulator buffers.
+// GEMM view per tile:  D[128 pixels, n_tile] += A[128 pixels, KCHUNK ch] * B[n_tile, KCHUNK ch]^T over taps x
+// channel chunks.  One TMA box per (tap, channel chunk), shifted by the tap offset, brings the activations into a
+// swizzled K-major ring slot next to the matching weight box; TMA out-of-bounds zero fill *is* the conv zero
+// padding, and the 128 GEMM rows may span several batch samples (4x4x8, 8x8x2).  Stride 2 walks every other input
+// pixel through TMA element strides.
 //
-// The same kernels run the plain convolutions of the encoders / PostProcess stack / BiSeNet (`epi == 1`:
+// conv_wgmma_kernel: persistent CTAs with a static schedule, three warpgroups.  Warpgroup 0 is the TMA producer
+// (one thread); warpgroups 1 and 2 each own 64 of the 128 GEMM rows, issue wgmma m64 x n_tile x k16 with the
+// fp32 accumulator in registers, release ring slots through mbarriers as their MMAs retire, and run the fused
+// epilogue: the accumulator goes through a padded fp32 staging tile in shared memory so that one thread sees
+// 32 consecutive channels of one pixel (two threads per pixel, alternating 32-channel chunks).  While the
+// consumers run an epilogue the producer is already filling the ring for their next tile.
+//
+// The same kernel runs the plain convolutions of the encoders / PostProcess stack / BiSeNet (`epi == 1`:
 // v = act(acc*scale[o] + shift[o]) (+ residual, before or after the activation), optional second output
-// v*s2[o] + b2[o] for the next block's BatchNorm; stride 2 through TMA element strides; grouped heads).
-//
-// Three kernels share the epilogues:
-//  * conv_halo2_kernel (cluster of 2, cta_group::2): the halo scheme below for N tile 256 with streamed weights;
-//    each CTA owns its own pixel tile and half of the weight tile, the leader issues M = 256 MMAs for the pair.
-//  * conv_halo_kernel (H % 16 == 0, W % 8 == 0): per 64-channel chunk ONE TMA 4-D box brings the
-//    (16+2) x (8+2)-pixel halo of an 8x16-pixel tile into a ring slot; the nine taps are nine UMMA
-//    descriptors that start (dy*pitch + dx) rows into that slot with SBO = one halo row (measured on
-//    B200: the 128B swizzle is a function of absolute smem address bits, so unaligned starts and a
-//    non-1024-multiple SBO are fine with base_offset = 0).  Each activation byte crosses L2->smem once
-//    per chunk instead of nine times.  Work is scheduled in ROUNDS of G consecutive tiles that share
-//    one 256-column accumulator buffer (G * n_tile <= 256), so narrow layers amortise every barrier /
-//    commit over the same amount of work as a wide one, and each weight tile is reused by G tiles.
-//    Weights either stay RESIDENT in smem for the whole kernel (single channel chunk, single N tile) or
-//    stream through their own TMA ring.  NG (2 or 4) 4-warp epilogue groups alternate rounds, one TMEM buffer each.
-//  * conv_igemm_kernel (any shape; used for 4^2 / 8^2, stride 2, 1x1, grouped): one TMA box per (tap, chunk)
-//    shifted by the tap offset; the 128 GEMM rows may span several batch samples (4x4x8, 8x8x2).
-// In all of them TMA out-of-bounds zero fill *is* the conv zero padding.
+// v*s2[o] + b2[o] for the next block's BatchNorm; stride 2; grouped heads).
 #include <stdlib.h>
 #include <string.h>
 
@@ -41,6 +33,7 @@
 namespace hf {
 
 constexpr int kMaxStages = 8;
+constexpr int kMaxDynSmem = 232448;   // 227 KB: opt-in dynamic shared memory per block on sm_90
 constexpr int kTableBytes = 16384;   // 512 entries x 32 B
 constexpr float kSqrt2 = 1.41421356237309515f;
 
@@ -49,16 +42,12 @@ struct ConvKernelParams {
   int Ho, Wo;
   int taps, up, act;
   int TW, TH, TB, tiles_x, tiles_y;
-  int n_tile, num_n_tiles, num_tiles;   // num_tiles = work items (tiles for v1, rounds x N tiles for halo)
+  int n_tile, num_n_tiles, num_tiles;   // num_tiles = work items (M tiles x N tiles)
   int num_m_tiles;
   int num_kb;              // taps * Cin / KCHUNK
   int kc_per_tap;          // Cin / KCHUNK
-  int stages;              // v1: A+B stages; halo: B stages (stream mode)
+  int stages;              // A+B ring stages
   uint32_t stage_bytes, a_bytes;
-  uint32_t idesc;
-  // halo kernel
-  int G, na_slots, pitch, b_resident;
-  uint32_t a_slot_bytes;
   const float* d;
   const float* noise;
   int64_t noise_bstride;
@@ -231,27 +220,35 @@ __device__ __forceinline__ void epi_chunk_enc(uint32_t ts, const uint32_t (&acc)
   }
 }
 
+// 32 accumulator columns [32q, 32q + 32) of one pixel row of the fp32 staging tile (conflict-free 16-byte reads:
+// the padded row pitch puts the eight rows of one shared-memory wavefront on different banks).
+__device__ __forceinline__ void load_acc_chunk(const float* srow, int q, uint32_t (&acc)[32]) {
+  const float4* s4 = reinterpret_cast<const float4*>(srow + q * 32);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 v = s4[i];
+    acc[4 * i] = __float_as_uint(v.x); acc[4 * i + 1] = __float_as_uint(v.y);
+    acc[4 * i + 2] = __float_as_uint(v.z); acc[4 * i + 3] = __float_as_uint(v.w);
+  }
+}
+
 // Encoder epilogue (plain conv + folded BatchNorm / bias + PReLU | LeakyReLU | ReLU + residual):
 //   v = act(acc*scale[o] + shift[o]) + residual ; y16 = v ; y16b = v*s2[o] + b2[o] ; y32 (NCHW) = v
 // (reference: bottleneck_IR_SE / IBasicBlock conv stacks, encoder4editing/models/encoders/helpers.py:98-120,
 //  FeatureStyleEncoder/arcface/iresnet.py:28-57; GradualStyleBlock psp_encoders.py:34-55)
-template <int DT, bool REMOTE_RELEASE>
-__device__ __forceinline__ void epilogue_tile_enc(const ConvKernelParams& p, const TableEntry* trow, uint32_t taddr,
-                                                  uint64_t* release_bar, int n0, int b, int y, int x, bool valid) {
+// Chunks q0, q0 + 2, ... of the pixel's row.
+template <int DT>
+__device__ __forceinline__ void epilogue_tile_enc(const ConvKernelParams& p, const TableEntry* trow, const float* srow,
+                                                  int q0, int n0, int b, int y, int x, bool valid) {
   const int chunks = p.n_tile / 32;
   const size_t plane_o = (size_t)p.Ho * p.Wo;
   const size_t pix = valid ? ((size_t)b * p.Ho + y) * p.Wo + x : 0;
   const uint32_t trow_s = smem_u32(trow);
   const int variant = p.out_nchw ? 3 : ((p.enc_residual ? 1 : 0) | (p.enc_y16b ? 2 : 0));
   const bool post = p.enc_post != 0;
-  for (int q = 0; q < chunks; ++q) {
+  for (int q = q0; q < chunks; q += 2) {
     uint32_t acc[32];
-    tmem_ld_32x32(taddr + q * 32, acc);
-    tmem_ld_wait();
-    if (release_bar && q == chunks - 1) {
-      tc_fence_before();
-      if (REMOTE_RELEASE) mbar_arrive_leader(release_bar); else mbar_arrive(release_bar);
-    }
+    load_acc_chunk(srow, q, acc);
     const int o_base = n0 + q * 32;
     const size_t eo = pix * p.Cout + o_base;
     const uint4* res = (p.enc_residual && valid) ? reinterpret_cast<const uint4*>(p.enc_residual + eo) : nullptr;
@@ -307,17 +304,16 @@ __device__ __forceinline__ void epi_chunk(uint32_t ts, const uint32_t (&acc)[32]
   }
 }
 
-// TMEM -> registers -> fused epilogue -> global, for one tile and one thread (= one GEMM row = one pixel).
+// staging tile -> fused epilogue -> global, for one pixel row and the chunks q0, q0 + 2, ... of it.
 //   a = acc*d + nw*noise + bias ; a = lrelu(a)*sqrt2 ; rgb += a*wrgb ; out16 = a*s_next
-// `release_bar` != nullptr: arrive on it right after the last TMEM read (hands the accumulator back).
-// The fused ToRGB partial sums exist for plain (non-upsampling) convolutions only (launch_conv checks).
-template <int DT, bool REMOTE_RELEASE = false>
-__device__ __forceinline__ void epilogue_tile(const ConvKernelParams& p, const TableEntry* trow, uint32_t taddr,
-                                              uint64_t* release_bar, int n0, int nt, int b, int y, int x, bool valid,
-                                              float4 nz, float nw) {
+// Returns this thread's share of the fused ToRGB dot products (plain, non-upsampling convolutions only;
+// launch_conv checks); the caller adds the two shares of a pixel.
+template <int DT>
+__device__ __forceinline__ float3 epilogue_tile(const ConvKernelParams& p, const TableEntry* trow, const float* srow,
+                                               int q0, int n0, int b, int y, int x, bool valid, float4 nz, float nw) {
   if (p.epi == 1) {
-    epilogue_tile_enc<DT, REMOTE_RELEASE>(p, trow, taddr, release_bar, n0, b, y, x, valid);
-    return;
+    epilogue_tile_enc<DT>(p, trow, srow, q0, n0, b, y, x, valid);
+    return make_float3(0.f, 0.f, 0.f);
   }
   const int chunks = p.n_tile / 32;
   const size_t plane_o = (size_t)p.Ho * p.Wo;
@@ -328,14 +324,9 @@ __device__ __forceinline__ void epilogue_tile(const ConvKernelParams& p, const T
   const uint32_t trow_s = smem_u32(trow);
   const int variant = (p.rgb_partial ? 1 : 0) | (p.out_nchw ? 2 : 0) | (p.xhat_out ? 4 : 0);
 
-  for (int q = 0; q < chunks; ++q) {
+  for (int q = q0; q < chunks; q += 2) {
     uint32_t acc[32];
-    tmem_ld_32x32(taddr + q * 32, acc);
-    tmem_ld_wait();
-    if (release_bar && q == chunks - 1) {
-      tc_fence_before();
-      if (REMOTE_RELEASE) mbar_arrive_leader(release_bar); else mbar_arrive(release_bar);
-    }
+    load_acc_chunk(srow, q, acc);
     if (p.dbg & 1) { r0 += __uint_as_float(acc[0]); continue; }
     const int par = p.up ? (q & 3) : 0;
     const int t_base = p.up ? (q >> 2) * 32 : q * 32;          // channel offset inside the tile
@@ -357,63 +348,56 @@ __device__ __forceinline__ void epilogue_tile(const ConvKernelParams& p, const T
       default: epi_chunk<DT, true, true, true>(ts, acc, nzv, slope, dst, r0, r1, r2, onchw, plane_o); break;
     }
   }
-  if (p.rgb_partial && valid) {
-    float* pp = p.rgb_partial + ((size_t)nt * p.B + b) * 3 * plane_o + (size_t)y * p.Wo + x;
-    pp[0] = r0; pp[plane_o] = r1; pp[2 * plane_o] = r2;
-  }
+  return make_float3(r0, r1, r2);
 }
 
 // =============================================================================================
-// v1: one TMA box per (tap, channel chunk)
+// conv_wgmma_kernel
 // =============================================================================================
-constexpr int kConvThreads = 192;
+constexpr int kConvThreads = 384;     // warpgroup 0: TMA producer; warpgroups 1, 2: MMA + epilogue, 64 rows each
+constexpr int kStagePad = 4;          // staging row pitch = n_tile + 4 floats
+constexpr int kMaxNTile = 128;        // m64 x n128 fp32 accumulator = 64 registers per thread
 
-template <int KCHUNK, int DT>
+// shared memory besides the ring: staging tiles, two epilogue tables, ToRGB exchange, barriers
+__host__ __device__ constexpr size_t conv_fixed_smem(int n_tile) {
+  return 1024 /*align*/ + (size_t)2 * 64 * (n_tile + kStagePad) * 4 + 2 * (size_t)kTableBytes + 2 * 64 * 4 * 4 +
+         2 * kMaxStages * 8;
+}
+
+template <int KCHUNK, int DT, int NT>
 __global__ void __launch_bounds__(kConvThreads, 1)
-conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const ConvKernelParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  constexpr int SP = NT + kStagePad;
   uint8_t* stage_base = smem;
-  TableEntry* table = reinterpret_cast<TableEntry*>(smem + (size_t)p.stages * p.stage_bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(table) + kTableBytes);
-  uint64_t* full_bar = bars;                       // [kMaxStages]
-  uint64_t* empty_bar = bars + kMaxStages;         // [kMaxStages]
-  uint64_t* tmem_full = bars + 2 * kMaxStages;     // [2]
-  uint64_t* tmem_empty = bars + 2 * kMaxStages + 2;  // [2]
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 4);
+  float* staging = reinterpret_cast<float*>(smem + (size_t)p.stages * p.stage_bytes);           // [2][64][SP]
+  TableEntry* tables = reinterpret_cast<TableEntry*>(staging + 2 * 64 * SP);                     // [2][512]
+  float* rgbx = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(tables) + 2 * kTableBytes);  // [2][64][4]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(rgbx + 2 * 64 * 4);                           // [kMaxStages]
+  uint64_t* empty_bar = full_bar + kMaxStages;                                                   // [kMaxStages]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   constexpr uint32_t ROW_BYTES = KCHUNK * 2;
   constexpr uint32_t SBO = 8 * ROW_BYTES;
-  constexpr uint32_t LAYOUT = (KCHUNK == 64) ? UMMA_LAYOUT_SW128 : UMMA_LAYOUT_SW64;
+  constexpr uint32_t LAYOUT = (KCHUNK == 64) ? GMMA_LAYOUT_SW128 : GMMA_LAYOUT_SW64;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 128);
+      mbar_init(&empty_bar[s], 8);                 // lane 0 of each of the eight consumer warps
     }
     mbar_fence_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_holder, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ================================ TMA producer ================================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       const int pad = (p.taps == 9) ? 1 : 0;
@@ -426,7 +410,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int tap = 0; tap < p.taps; ++tap) {
           const int dy = (p.taps == 9) ? tap / 3 : 0, dx = (p.taps == 9) ? tap % 3 : 0;
           for (int kc = 0; kc < p.kc_per_tap; ++kc) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
+            mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
             uint8_t* a_dst = stage_base + (size_t)stage * p.stage_bytes;
             uint8_t* b_dst = a_dst + p.a_bytes;
             mbar_expect_tx(&full_bar[stage], tx_bytes);
@@ -439,491 +423,93 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ==================================
-    // one elected lane runs the whole main loop (see conv_halo_kernel)
-    if (elect_one()) {
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    const uint32_t smem_base_u32 = smem_u32(stage_base);
-    const uint32_t desc_hi = kmajor_desc_hi(SBO, LAYOUT);
-    const uint32_t idesc = p.idesc;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-      const int buf = it & 1;
-      const uint32_t use = (uint32_t)(it >> 1);
-      mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(buf * 256);
-      for (int kb = 0; kb < p.num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        {
-          const uint32_t a_addr = smem_base_u32 + (uint32_t)stage * p.stage_bytes;
-          const uint32_t b_addr = a_addr + p.a_bytes;
-          umma_tap<KCHUNK / 16>(tmem_d, kmajor_desc_lo(a_addr), desc_hi, kmajor_desc_lo(b_addr), desc_hi, idesc,
-                                kb > 0 ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);                    // frees the smem slot when the MMAs retire
-          if (kb == p.num_kb - 1) umma_commit(&tmem_full[buf]);   // accumulator ready for the epilogue
-        }
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-    }
-    }  // elect_one
-  } else {
-    // ================================ epilogue (4 warps) ==========================
-    const int wq = warp & 3;                 // TMEM lane quarter this warp may read
-    const int row = wq * 32 + lane;          // GEMM row = pixel within the tile
-    const int etid = (warp - 2) * 32 + lane; // 0..127
-    const int w_l = row % p.TW, h_l = (row / p.TW) % p.TH, bb = row / (p.TW * p.TH);
-    const float nw = p.noise_w ? __ldg(p.noise_w) : 0.f;
-    const int nc_tile = p.up ? p.n_tile / 4 : p.n_tile;
-    int it = 0;
-    int cached_bt = -1, cached_nt = -1;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-      const int nt = tile % p.num_n_tiles;
-      const MTile tc = decode_mtile(p, tile / p.num_n_tiles);
-      const int x = tc.x0 + w_l, y = tc.y0 + h_l, b = tc.bt * p.TB + bb;
-      const int n0 = nt * p.n_tile;
-      const bool valid = b < p.B;
-      if (tc.bt != cached_bt || nt != cached_nt) {     // table depends on (batch tile, N tile) only
-        named_bar_sync(1, 128);
-        fill_table(p, table, etid, tc.bt, n0);
-        named_bar_sync(1, 128);
-        cached_bt = tc.bt; cached_nt = nt;
-      }
-      const float4 nz = valid ? load_noise(p, b, y, x, nw) : make_float4(0.f, 0.f, 0.f, 0.f);
-      const int buf = it & 1;
-      const uint32_t use = (uint32_t)(it >> 1);
-      mbar_wait(&tmem_full[buf], use & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)(buf * 256);
-      epilogue_tile<DT>(p, table + (p.epi == 1 ? 0 : bb * nc_tile), taddr, &tmem_empty[buf], n0, nt, b, y, x, valid, nz, nw);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // ================================ consumers: MMA + epilogue ============================
+  const int cg = (threadIdx.x >> 7) - 1;       // GEMM rows [64 cg, 64 cg + 64)
+  const int t = threadIdx.x & 127;
+  const int cw = t >> 5;                       // warp within the warpgroup: accumulator rows [16 cw, 16 cw + 16)
+  const int bar_id = 1 + cg;
+  float* stg = staging + cg * 64 * SP;
+  TableEntry* table = tables + cg * (kTableBytes / (int)sizeof(TableEntry));
+  float* rx = rgbx + cg * 64 * 4;
+  // epilogue: two threads per pixel row (t and t + 64), alternating 32-channel chunks
+  const int er = t & 63, half = t >> 6;
+  const int row = cg * 64 + er;
+  const int w_l = row % p.TW, h_l = (row / p.TW) % p.TH, bb = row / (p.TW * p.TH);
+  const float nw = p.noise_w ? __ldg(p.noise_w) : 0.f;
+  const int nc_tile = p.up ? p.n_tile / 4 : p.n_tile;
+  const size_t plane_o = (size_t)p.Ho * p.Wo;
+  const uint32_t a_off = (uint32_t)cg * 64u * ROW_BYTES;
+  const uint32_t smem_base_u32 = smem_u32(stage_base);
+  int stage = 0;
+  uint32_t phase = 0;
+  int cached_bt = -1, cached_nt = -1;
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const int nt = tile % p.num_n_tiles;
+    const MTile tc = decode_mtile(p, tile / p.num_n_tiles);
+    const int x = tc.x0 + w_l, y = tc.y0 + h_l, b = tc.bt * p.TB + bb;
+    const int n0 = nt * p.n_tile;
+    const bool valid = b < p.B;
+    if (tc.bt != cached_bt || nt != cached_nt) {     // table depends on (batch tile, N tile) only
+      named_bar_sync(bar_id, 128);
+      fill_table(p, table, t, tc.bt, n0);
+      named_bar_sync(bar_id, 128);
+      cached_bt = tc.bt; cached_nt = nt;
+    }
+    const float4 nz = valid ? load_noise(p, b, y, x, nw) : make_float4(0.f, 0.f, 0.f, 0.f);
+
+    float acc[NT / 2];
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < p.num_kb; ++kb) {
+      mbar_wait_nocall(&full_bar[stage], phase);
+      const uint32_t a_addr = smem_base_u32 + (uint32_t)stage * p.stage_bytes;
+      const uint64_t da = make_gmma_desc(a_addr + a_off, SBO, LAYOUT);
+      const uint64_t db = make_gmma_desc(a_addr + p.a_bytes, SBO, LAYOUT);
+      wgmma_fence_regs(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < KCHUNK / 16; ++k) Wgmma<NT, DT>::mma(acc, da + 2 * k, db + 2 * k);
+      wgmma_commit();
+      wgmma_fence_regs(acc);
+      wgmma_wait<1>();                              // the previous k-block's MMAs have retired: free its slot
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == p.stages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+
+    // accumulator fragment -> staging rows (m64nNk16: row 16*warp + lane/4 (+8), columns 8j + 2*(lane%4) (+1))
+    {
+      const int r0 = cw * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) {
+        *reinterpret_cast<float2*>(stg + r0 * SP + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(stg + (r0 + 8) * SP + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+    }
+    named_bar_sync(bar_id, 128);
+    const float3 r = epilogue_tile<DT>(p, table + (p.epi == 1 ? 0 : bb * nc_tile), stg + er * SP, half, n0, b, y, x,
+                                       valid, nz, nw);
+    if (p.rgb_partial && half) { rx[er * 4] = r.x; rx[er * 4 + 1] = r.y; rx[er * 4 + 2] = r.z; }
+    named_bar_sync(bar_id, 128);                   // staging tile and ToRGB shares consumed
+    if (p.rgb_partial && !half && valid) {
+      float* pp = p.rgb_partial + ((size_t)nt * p.B + b) * 3 * plane_o + (size_t)y * p.Wo + x;
+      pp[0] = r.x + rx[er * 4]; pp[plane_o] = r.y + rx[er * 4 + 1]; pp[2 * plane_o] = r.z + rx[er * 4 + 2];
+    }
   }
 }
-
-// =============================================================================================
-// halo kernel: halo tile ring in smem, nine taps = nine shifted UMMA descriptors, rounds of G tiles
-// =============================================================================================
-constexpr int kHaloThreads = 320;      // warp 0 TMA, warp 1 MMA, warps 2-5 / 6-9 two epilogue groups
-constexpr int kHaloTW = 8, kHaloTH = 16;
-constexpr int kHaloRows = kHaloTH + 2;
-constexpr int kHaloPitch = kHaloTW + 2;   // dense halo rows (pitch 16 measured no faster)
-constexpr int kMaxASlots = 8;
-constexpr int kMaxG = 8;
-
-// NG = number of epilogue groups (4 warps each) = number of TMEM accumulator buffers of 512/NG columns.  NG = 4
-// (576 threads, <= 112 registers) serves the resident-weight low-channel layers, whose per-tile MMA time is shorter
-// than what two groups need for the epilogue (ncu: 2 epilogue warps per SM sub-partition issue 28 % of the time).
-template <int KCHUNK, int DT, int NG>
-__global__ void __launch_bounds__(64 + 128 * NG, 1)
-conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const ConvKernelParams p) {
-  constexpr int BUF_COLS = 512 / NG;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr uint32_t ROW_BYTES = KCHUNK * 2;
-  constexpr uint32_t SBO_B = 8 * ROW_BYTES;
-  constexpr uint32_t LAYOUT = (KCHUNK == 64) ? UMMA_LAYOUT_SW128 : UMMA_LAYOUT_SW64;
-  const uint32_t a_slot = p.a_slot_bytes;
-  const uint32_t a_tx = (uint32_t)kHaloRows * kHaloPitch * ROW_BYTES;     // bytes one halo box delivers
-  const uint32_t tap_bytes = (uint32_t)p.n_tile * ROW_BYTES;           // one tap of weights
-  const int b_slots = p.b_resident ? 9 : p.stages;
-  uint8_t* a_base = smem;                                              // [na_slots][a_slot]
-  uint8_t* b_base = smem + (size_t)p.na_slots * a_slot;                // [b_slots][tap_bytes]
-  TableEntry* table = reinterpret_cast<TableEntry*>(b_base + (size_t)b_slots * tap_bytes);   // 2 x 8 KB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(table) + kTableBytes);
-  uint64_t* b_full = bars;                          // [kMaxStages]
-  uint64_t* b_empty = b_full + kMaxStages;          // [kMaxStages]
-  uint64_t* a_full = b_empty + kMaxStages;          // [kMaxASlots]
-  uint64_t* a_empty = a_full + kMaxASlots;          // [kMaxASlots]
-  uint64_t* tmem_full = a_empty + kMaxASlots;       // [NG]
-  uint64_t* tmem_empty = tmem_full + 4;             // [NG]
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_empty + 4);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int G = p.G, NA = p.na_slots;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int s = 0; s < kMaxStages; ++s) {
-      mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], 1);
-    }
-    for (int i = 0; i < kMaxASlots; ++i) {
-      mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
-    }
-    for (int i = 0; i < NG; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 128);
-    }
-    mbar_fence_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_holder, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-
-  if (warp == 0) {
-    // ================================ TMA producer ================================
-    if (lane == 0) {
-      int bs = 0, as = 0;
-      uint32_t bphase = 0, aphase = 0;
-      if (p.b_resident) {                    // whole weight matrix of this layer: loaded once, never released
-        mbar_expect_tx(&b_full[0], 9 * tap_bytes);
-        for (int tap = 0; tap < 9; ++tap)
-          tma_load_2d(b_base + (size_t)tap * tap_bytes, &tmB, &b_full[0], tap * p.cin_g, 0);
-      }
-      for (int w = blockIdx.x; w < p.num_tiles; w += gridDim.x) {
-        const int nt = w % p.num_n_tiles, m0 = (w / p.num_n_tiles) * G;
-        const int gcount = min(G, p.num_m_tiles - m0);
-        const int n0 = nt * p.n_tile;
-        const int c_off = (n0 / p.cout_g) * p.cin_g;
-        for (int kc = 0; kc < p.kc_per_tap; ++kc) {
-          for (int g = 0; g < gcount; ++g) {
-            const MTile tc = decode_mtile(p, m0 + g);
-            mbar_wait(&a_empty[as], aphase ^ 1);
-            mbar_expect_tx(&a_full[as], a_tx);
-            tma_load_4d(a_base + (size_t)as * a_slot, &tmA, &a_full[as], c_off + kc * KCHUNK, tc.x0 - 1, tc.y0 - 1, tc.bt);
-            if (++as == NA) { as = 0; aphase ^= 1; }
-          }
-          if (!p.b_resident) {
-            for (int tap = 0; tap < 9; ++tap) {
-              mbar_wait(&b_empty[bs], bphase ^ 1);
-              mbar_expect_tx(&b_full[bs], tap_bytes);
-              tma_load_2d(b_base + (size_t)bs * tap_bytes, &tmB, &b_full[bs], tap * p.cin_g + kc * KCHUNK, n0);
-              if (++bs == p.stages) { bs = 0; bphase ^= 1; }
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ==================================
-    // CUTLASS style: ONE elected lane runs the whole main loop (waits, MMAs, commits); the other 31 lanes go
-    // straight to the final barrier.  Measured: ~150 issue cycles per UTCHMMA with per-instruction elect.
-    if (elect_one()) {
-    int bs = 0, as = 0;
-    uint32_t bphase = 0, aphase = 0;
-    int it = 0;
-    constexpr int NK = KCHUNK / 16;
-    constexpr uint32_t ROW_LO = ROW_BYTES >> 4;                      // one halo pixel row in descriptor units
-    const uint32_t a_base_lo = kmajor_desc_lo(smem_u32(a_base)), b_base_lo = kmajor_desc_lo(smem_u32(b_base));
-    const uint32_t a_slot_lo = a_slot >> 4, tap_lo = tap_bytes >> 4;
-    constexpr uint32_t SBO_A = kHaloPitch * ROW_BYTES;               // next 8-pixel group = next halo row
-    const uint32_t hi_a = kmajor_desc_hi(SBO_A, LAYOUT), hi_b = kmajor_desc_hi(SBO_B, LAYOUT);
-    const uint32_t idesc = p.idesc;
-    const uint32_t n_tile = (uint32_t)p.n_tile;
-    if (p.b_resident) {
-      mbar_wait(&b_full[0], 0);
-      tc_fence_after();
-    }
-    for (int w = blockIdx.x; w < p.num_tiles; w += gridDim.x, ++it) {
-      const int m0 = (w / p.num_n_tiles) * G;
-      const int gcount = min(G, p.num_m_tiles - m0);
-      const int buf = it % NG;
-      const uint32_t use = (uint32_t)(it / NG);
-      mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(buf * BUF_COLS);
-      if (p.b_resident) {
-        // order (tile g, tap): each halo slot is released as soon as its nine taps are issued
-        for (int g = 0; g < gcount; ++g) {
-          mbar_wait(&a_full[as], aphase);
-          tc_fence_after();
-          const uint32_t a_lo = a_base_lo + (uint32_t)as * a_slot_lo;
-          const uint32_t d_addr = tmem_d + (uint32_t)g * n_tile;
-          // rolled on purpose: the single issuing warp must stay inside the instruction cache
-          // (the fully unrolled form measured ~2x slower: its stalls were all `no_inst`)
-          uint32_t b_lo = b_base_lo;
-#pragma unroll 1
-          for (int dy = 0; dy < 3; ++dy) {
-#pragma unroll 1
-            for (int dx = 0; dx < 3; ++dx) {
-              umma_tap<NK>(d_addr, a_lo + (uint32_t)(dy * kHaloPitch + dx) * ROW_LO, hi_a, b_lo, hi_b, idesc,
-                                (dy | dx) ? 1u : 0u);
-              b_lo += tap_lo;
-            }
-          }
-          umma_commit(&a_empty[as]);
-          if (++as == NA) { as = 0; aphase ^= 1; }
-        }
-        umma_commit(&tmem_full[buf]);
-      } else {
-        // order (chunk, tap, tile g): every streamed weight tile is used by all G tiles of the round
-        for (int kc = 0; kc < p.kc_per_tap; ++kc) {
-          {
-            int s = as;
-            uint32_t ph = aphase;
-            for (int g = 0; g < gcount; ++g) {
-              mbar_wait(&a_full[s], ph);
-              if (++s == NA) { s = 0; ph ^= 1; }
-            }
-          }
-#pragma unroll 1
-          for (int tap = 0; tap < 9; ++tap) {
-            mbar_wait(&b_full[bs], bphase);
-            tc_fence_after();
-            const uint32_t b_lo = b_base_lo + (uint32_t)bs * tap_lo;
-            const int dy = tap / 3;
-            const uint32_t tap_off = (uint32_t)(dy * kHaloPitch + (tap - 3 * dy)) * ROW_LO;
-            const uint32_t acc = (kc > 0 || tap > 0) ? 1u : 0u;
-            int s = as;
-            for (int g = 0; g < gcount; ++g) {
-              umma_tap<NK>(tmem_d + (uint32_t)g * n_tile, a_base_lo + (uint32_t)s * a_slot_lo + tap_off, hi_a, b_lo,
-                                hi_b, idesc, acc);
-              if (++s == NA) s = 0;
-            }
-            umma_commit(&b_empty[bs]);
-            if (++bs == p.stages) { bs = 0; bphase ^= 1; }
-          }
-          for (int g = 0; g < gcount; ++g) {
-            umma_commit(&a_empty[as]);
-            if (++as == NA) { as = 0; aphase ^= 1; }
-          }
-        }
-        umma_commit(&tmem_full[buf]);
-      }
-    }
-    }  // elect_one
-  } else {
-    // ================================ epilogue: NG groups of 4 warps ===============
-    const int grp = (warp - 2) >> 2;         // group g owns TMEM buffer g and the rounds with it % NG == g
-    const int wq = warp & 3;
-    const int row = wq * 32 + lane;
-    const int etid = ((warp - 2) & 3) * 32 + lane;
-    const int w_l = row & (kHaloTW - 1), h_l = row >> 3;
-    const float nw = p.noise_w ? __ldg(p.noise_w) : 0.f;
-    TableEntry* my_table = table + grp * BUF_COLS;
-    int cached_bt = -1, cached_nt = -1;
-    int it = 0;
-    uint32_t use = 0;
-    for (int w = blockIdx.x; w < p.num_tiles; w += gridDim.x, ++it) {
-      if ((it % NG) != grp) continue;
-      const int nt = w % p.num_n_tiles, m0 = (w / p.num_n_tiles) * G;
-      const int gcount = min(G, p.num_m_tiles - m0);
-      const int n0 = nt * p.n_tile;
-      MTile tc = decode_mtile(p, m0);
-      float4 nz_next = load_noise(p, tc.bt, tc.y0 + h_l, tc.x0 + w_l, nw);   // overlaps the MMAs of this round
-      mbar_wait(&tmem_full[grp], use & 1);
-      ++use;
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)(grp * BUF_COLS);
-      for (int g = 0; g < gcount; ++g) {
-        const float4 nz = nz_next;
-        const MTile cur = tc;
-        if (g + 1 < gcount) {
-          tc = decode_mtile(p, m0 + g + 1);
-          nz_next = load_noise(p, tc.bt, tc.y0 + h_l, tc.x0 + w_l, nw);
-        }
-        if (cur.bt != cached_bt || nt != cached_nt) {
-          named_bar_sync(1 + grp, 128);
-          fill_table(p, my_table, etid, cur.bt, n0);
-          named_bar_sync(1 + grp, 128);
-          cached_bt = cur.bt; cached_nt = nt;
-        }
-        epilogue_tile<DT>(p, my_table, taddr + (uint32_t)(g * p.n_tile), g == gcount - 1 ? &tmem_empty[grp] : nullptr,
-                          n0, nt, cur.bt, cur.y0 + h_l, cur.x0 + w_l, true, nz, nw);
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// =============================================================================================
-// halo kernel, CTA-pair form (cta_group::2) for the wide layers (N tile 256, streamed weights, G = 1):
-// two CTAs of a cluster each own one 8x16-pixel tile (their own halo ring and accumulator) and HALF of the
-// 256-row weight tile; the leader issues M=256 x N=256 x K=16 tcgen05.mma for both.  The ~130-cycle fixed
-// cost that every SS-mode MMA pays (measured, profiles/) is paid once per two tiles, and each CTA pulls
-// only half of the weights through L2 -> smem.
-// =============================================================================================
-template <int DT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kHaloThreads, 1)
-conv_halo2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const ConvKernelParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr int KCHUNK = 64;
-  constexpr uint32_t ROW_BYTES = KCHUNK * 2;
-  constexpr uint32_t ROW_LO = ROW_BYTES >> 4;
-  constexpr uint32_t SBO_A = kHaloPitch * ROW_BYTES, SBO_B = 8 * ROW_BYTES;
-  constexpr uint32_t LAYOUT = UMMA_LAYOUT_SW128;
-  constexpr uint32_t A_TX = kHaloRows * kHaloPitch * ROW_BYTES;
-  constexpr uint32_t B_HALF = 128 * ROW_BYTES;                        // this CTA's half of one weight tap
-  const uint32_t a_slot = p.a_slot_bytes;
-  const int NA = p.na_slots, NS = p.stages;
-  uint8_t* a_base = smem;
-  uint8_t* b_base = smem + (size_t)NA * a_slot;
-  TableEntry* table = reinterpret_cast<TableEntry*>(b_base + (size_t)NS * B_HALF);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(table) + kTableBytes);
-  uint64_t* b_full = bars;                          // leader's copies are the ones waited on
-  uint64_t* b_empty = b_full + kMaxStages;
-  uint64_t* a_full = b_empty + kMaxStages;
-  uint64_t* a_empty = a_full + kMaxASlots;
-  uint64_t* tmem_full = a_empty + kMaxASlots;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int s = 0; s < kMaxStages; ++s) {
-      mbar_init(&b_full[s], 2);                     // leader's expect_tx arrive + peer's arrive
-      mbar_init(&b_empty[s], 1);                    // leader's multicast commit
-    }
-    for (int i = 0; i < kMaxASlots; ++i) {
-      mbar_init(&a_full[i], 2);
-      mbar_init(&a_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);                  // multicast commit
-      mbar_init(&tmem_empty[i], 256);               // epilogue threads of both CTAs
-    }
-    mbar_fence_init();
-  }
-  if (warp == 1) {
-    tmem_alloc2(tmem_holder, 512);
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-
-  // work item w (per pair): N tile nt, pair round pr -> this CTA's tile = 2*pr + rank
-  if (warp == 0) {
-    // ================================ TMA producer (both CTAs) ====================
-    if (lane == 0) {
-      int bs = 0, as = 0;
-      uint32_t bphase = 0, aphase = 0;
-      for (int w = pair; w < p.num_tiles; w += num_pairs) {
-        const int nt = w % p.num_n_tiles;
-        const MTile tc = decode_mtile(p, 2 * (w / p.num_n_tiles) + (int)rank);
-        const int n0 = nt * 256 + (int)rank * 128;
-        const int c_off = ((nt * 256) / p.cout_g) * p.cin_g;
-        for (int kc = 0; kc < p.kc_per_tap; ++kc) {
-          mbar_wait(&a_empty[as], aphase ^ 1);
-          if (leader) mbar_expect_tx(&a_full[as], 2 * A_TX); else mbar_arrive_leader(&a_full[as]);
-          tma2_load_4d(a_base + (size_t)as * a_slot, &tmA, &a_full[as], c_off + kc * KCHUNK, tc.x0 - 1, tc.y0 - 1, tc.bt);
-          if (++as == NA) { as = 0; aphase ^= 1; }
-          for (int tap = 0; tap < 9; ++tap) {
-            mbar_wait(&b_empty[bs], bphase ^ 1);
-            if (leader) mbar_expect_tx(&b_full[bs], 2 * B_HALF); else mbar_arrive_leader(&b_full[bs]);
-            tma2_load_2d(b_base + (size_t)bs * B_HALF, &tmB, &b_full[bs], tap * p.cin_g + kc * KCHUNK, n0);
-            if (++bs == NS) { bs = 0; bphase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================================ MMA issuer (leader CTA, one elected lane) ====
-    if (leader && elect_one()) {
-      int bs = 0, as = 0;
-      uint32_t bphase = 0, aphase = 0;
-      int it = 0;
-      const uint32_t a_base_lo = kmajor_desc_lo(smem_u32(a_base)), b_base_lo = kmajor_desc_lo(smem_u32(b_base));
-      const uint32_t a_slot_lo = a_slot >> 4, b_half_lo = B_HALF >> 4;
-      const uint32_t hi_a = kmajor_desc_hi(SBO_A, LAYOUT), hi_b = kmajor_desc_hi(SBO_B, LAYOUT);
-      const uint32_t idesc = p.idesc;
-      for (int w = pair; w < p.num_tiles; w += num_pairs, ++it) {
-        const int buf = it & 1;
-        const uint32_t use = (uint32_t)(it >> 1);
-        mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(buf * 256);
-        for (int kc = 0; kc < p.kc_per_tap; ++kc) {
-          mbar_wait(&a_full[as], aphase);
-          const uint32_t a_lo = a_base_lo + (uint32_t)as * a_slot_lo;
-#pragma unroll 1
-          for (int tap = 0; tap < 9; ++tap) {
-            mbar_wait(&b_full[bs], bphase);
-            tc_fence_after();
-            const int dy = tap / 3;
-            umma_tap2_x4(tmem_d, a_lo + (uint32_t)(dy * kHaloPitch + (tap - 3 * dy)) * ROW_LO, hi_a,
-                         b_base_lo + (uint32_t)bs * b_half_lo, hi_b, idesc, (kc > 0 || tap > 0) ? 1u : 0u);
-            umma_commit2(&b_empty[bs]);
-            if (++bs == NS) { bs = 0; bphase ^= 1; }
-          }
-          umma_commit2(&a_empty[as]);
-          if (++as == NA) { as = 0; aphase ^= 1; }
-        }
-        umma_commit2(&tmem_full[buf]);
-      }
-    }
-  } else {
-    // ================================ epilogue: two groups of 4 warps (both CTAs) ==
-    const int grp = (warp - 2) >> 2;
-    const int wq = warp & 3;
-    const int row = wq * 32 + lane;
-    const int etid = ((warp - 2) & 3) * 32 + lane;
-    const int w_l = row & (kHaloTW - 1), h_l = row >> 3;
-    const float nw = p.noise_w ? __ldg(p.noise_w) : 0.f;
-    TableEntry* my_table = table + grp * 256;
-    int cached_bt = -1, cached_nt = -1;
-    int it = 0;
-    uint32_t use = 0;
-    for (int w = pair; w < p.num_tiles; w += num_pairs, ++it) {
-      if ((it & 1) != grp) continue;
-      const int nt = w % p.num_n_tiles;
-      const MTile tc = decode_mtile(p, 2 * (w / p.num_n_tiles) + (int)rank);
-      const int n0 = nt * 256;
-      const float4 nz = load_noise(p, tc.bt, tc.y0 + h_l, tc.x0 + w_l, nw);
-      if (tc.bt != cached_bt || nt != cached_nt) {
-        named_bar_sync(1 + grp, 128);
-        fill_table(p, my_table, etid, tc.bt, n0);
-        named_bar_sync(1 + grp, 128);
-        cached_bt = tc.bt; cached_nt = nt;
-      }
-      mbar_wait(&tmem_full[grp], use & 1);
-      ++use;
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)(grp * 256);
-      // hand the accumulator back to the LEADER's barrier (remote arrive from the peer CTA)
-      epilogue_tile<DT, true>(p, my_table, taddr, &tmem_empty[grp], n0, nt, tc.bt, tc.y0 + h_l, tc.x0 + w_l, true, nz, nw);
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();       // the peer's smem / TMEM are read by the leader's MMAs until the very end
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, 512);
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
 int conv_up_nc(int Cout) { return Cout < 32 ? Cout : 32; }
 
-// Experiment knobs (HF_CONV_V1: force the v1 kernel; HF_CONV_DBG: drop the epilogue -> WRONG outputs) exist only in
+// Experiment knobs (HF_CONV_DBG: drop the epilogue -> WRONG outputs) exist only in
 // -DHF_DEBUG builds; the shipped library never reads the environment on the launch path.
 #ifdef HF_DEBUG
 static int env_int(const char* name, int dflt) {
@@ -948,17 +534,12 @@ int conv_plan(const ConvLaunch& a, ConvPlan* p) {
   HF_REQUIRE(stride == 1 || (a.H % 2 == 0 && a.W % 2 == 0) || (a.H == 1 && a.W == 1), "conv: stride 2 needs even H, W");
   // the GEMM rows are OUTPUT pixels (input pixels for the polyphase up-conv)
   const int MH = stride == 2 ? (a.H + 1) / 2 : a.H, MW = stride == 2 ? (a.W + 1) / 2 : a.W;
-  p->halo = (a.taps == 9 && stride == 1 && a.H % kHaloTH == 0 && a.W % kHaloTW == 0 && !env_int("HF_CONV_V1", 0)) ? 1 : 0;
-  p->G = 1; p->na_slots = 0; p->pitch = 0; p->b_resident = 0; p->a_slot_bytes = 0; p->ng = 2;
-  if (p->halo) {
-    p->TW = kHaloTW; p->TH = kHaloTH; p->TB = 1;
-  } else {
-    p->TW = MW < 16 ? MW : 16;
-    HF_REQUIRE(128 % p->TW == 0, "conv: width %d unsupported (tile width must divide 128)", MW);
-    p->TH = MH < 128 / p->TW ? MH : 128 / p->TW;
-    HF_REQUIRE(128 % (p->TW * p->TH) == 0, "conv: %dx%d image does not tile into 128 GEMM rows", MH, MW);
-    p->TB = 128 / (p->TW * p->TH);
-  }
+  p->halo = 0; p->G = 1; p->na_slots = 0; p->pitch = 0; p->b_resident = 0; p->a_slot_bytes = 0; p->ng = 2;
+  p->TW = MW < 16 ? MW : 16;
+  HF_REQUIRE(128 % p->TW == 0, "conv: width %d unsupported (tile width must divide 128)", MW);
+  p->TH = MH < 128 / p->TW ? MH : 128 / p->TW;
+  HF_REQUIRE(128 % (p->TW * p->TH) == 0, "conv: %dx%d image does not tile into 128 GEMM rows", MH, MW);
+  p->TB = 128 / (p->TW * p->TH);
   HF_REQUIRE(MW % p->TW == 0 && MH % p->TH == 0, "conv: %dx%d not divisible by tile %dx%d", MH, MW, p->TH, p->TW);
   p->tiles_x = MW / p->TW;
   p->tiles_y = MH / p->TH;
@@ -969,130 +550,47 @@ int conv_plan(const ConvLaunch& a, ConvPlan* p) {
   const int cout_g = ntot / groups;                  // an N tile never straddles two groups
   const int nmin = a.up ? 128 : 32;
   const int sms = num_sms();
-  const int table_cap = p->halo ? 256 : 512;       // entries per epilogue group
+  const int table_cap = kTableBytes / (int)sizeof(TableEntry);   // entries per consumer warpgroup
   const int tb_rows = a.epi == 1 ? 1 : p->TB;      // encoder epilogue tables are per channel only
   int n_tile = 0;
   if (a.force_n_tile) {
     n_tile = a.force_n_tile;
   } else {
-    for (int cand = 256; cand >= nmin; cand >>= 1) {
+    for (int cand = kMaxNTile; cand >= nmin; cand >>= 1) {
       if (cout_g % cand || tb_rows * (a.up ? cand / 4 : cand) > table_cap) continue;
       n_tile = cand;
       if ((int64_t)p->num_m_tiles * (ntot / cand) >= sms) break;   // largest tile that still fills the GPU
     }
   }
-  HF_REQUIRE(n_tile >= nmin && n_tile <= 256 && cout_g % n_tile == 0 && n_tile % 32 == 0 &&
+  HF_REQUIRE(n_tile >= nmin && n_tile <= kMaxNTile && cout_g % n_tile == 0 && n_tile % 32 == 0 &&
                  tb_rows * (a.up ? n_tile / 4 : n_tile) <= table_cap,
              "conv: no valid N tile (Ntot=%d, n_tile=%d, TB=%d)", ntot, n_tile, p->TB);
   p->n_tile = n_tile;
   p->num_n_tiles = ntot / n_tile;
   p->nc = a.up ? n_tile / 4 : n_tile;
-  const size_t fixed = 1024 /*align*/ + kTableBytes + 512 /*barriers*/;
-  const size_t budget = 232448 - fixed;
+  const size_t fixed = conv_fixed_smem(n_tile);
+  const size_t budget = kMaxDynSmem - fixed;
   const int row_bytes = p->kchunk * 2;
-  if (p->halo) {
-    p->pitch = kHaloPitch;
-    p->a_slot_bytes = (uint32_t)(((size_t)kHaloRows * p->pitch * row_bytes + 1023) & ~size_t(1023));
-    const size_t tap_bytes = (size_t)n_tile * row_bytes;
-    const int kc = cin_g / p->kchunk;
-    p->b_resident = (kc == 1 && p->num_n_tiles == 1 && 9 * tap_bytes + 2 * (size_t)p->a_slot_bytes <= budget &&
-                     env_int("HF_HALO_RESIDENT", 1))
-                        ? 1 : 0;
-    // epilogue groups / accumulator buffers: the 32-channel resident-weight layers (18 MMAs per tile) are
-    // epilogue-bound with two groups and get four buffers of 128 columns and four groups.  Measured (B=4, us,
-    // NG=2 -> NG=4): 32->32@1024^2 220 -> 203, but 64->64@512^2 115 -> 125 and 64->32 up 154 -> 172 (smaller
-    // rounds, 96-register budget), so wider layers keep two groups.
-    p->ng = (p->b_resident && n_tile == 32 && env_int("HF_HALO_NG", 4) == 4) ? 4 : 2;
-    const int buf_cols = 512 / p->ng;
-    // rounds: G tiles share one accumulator buffer; keep at least one round per SM
-    int G = 1;
-    const int gmax = env_int("HF_HALO_GMAX", kMaxG);
-    while (G * 2 <= gmax && G * 2 * n_tile <= buf_cols &&
-           (int64_t)(p->num_m_tiles / (G * 2)) * p->num_n_tiles >= sms)
-      G *= 2;
-    p->G = G;
-    if (p->b_resident) {
-      int na = (int)((budget - 9 * tap_bytes) / p->a_slot_bytes);
-      p->na_slots = na > kMaxASlots ? kMaxASlots : na;
-      p->stages = 1;
-      p->smem_bytes = fixed + 9 * tap_bytes + (size_t)p->na_slots * p->a_slot_bytes;
-    } else {
-      // A ring: 2G slots if they fit next to >= 3 weight stages, else G
-      int na = 2 * G;
-      if ((size_t)na * p->a_slot_bytes + 3 * tap_bytes > budget) na = G;
-      if (na > kMaxASlots) na = kMaxASlots;
-      if (na < 2) na = 2;
-      HF_REQUIRE(na >= G, "conv: halo ring too small for G=%d", G);
-      int stages = (int)((budget - (size_t)na * p->a_slot_bytes) / tap_bytes);
-      if (stages > kMaxStages) stages = kMaxStages;
-      HF_REQUIRE(stages >= 2, "conv: not enough shared memory for 2 weight stages");
-      // spend what is left on more halo slots
-      while (na < kMaxASlots && (size_t)(na + 1) * p->a_slot_bytes + (size_t)stages * tap_bytes <= budget) ++na;
-      if (env_int("HF_HALO_NA", 0) >= G) na = env_int("HF_HALO_NA", 0);             // tuning knobs
-      if (env_int("HF_HALO_STAGES", 0) >= 2 && env_int("HF_HALO_STAGES", 0) <= stages) stages = env_int("HF_HALO_STAGES", 0);
-      p->na_slots = na;
-      p->stages = stages;
-      p->smem_bytes = fixed + (size_t)na * p->a_slot_bytes + (size_t)stages * tap_bytes;
-    }
-    const int rounds = (p->num_m_tiles + G - 1) / G;
-    p->num_tiles = rounds * p->num_n_tiles;
-    // CTA-pair form for the wide layers: N tile 256 (128 weight rows per CTA), streamed weights, G = 1
-    if (!p->b_resident && G == 1 && n_tile == 256 && p->kchunk == 64 && p->num_m_tiles % 2 == 0 && sms % 2 == 0 &&
-        env_int("HF_CONV_2CTA", 1)) {
-      p->halo = 2;
-      const size_t half = (size_t)128 * row_bytes;
-      int na = 3;
-      int stages = (int)((budget - (size_t)na * p->a_slot_bytes) / half);
-      if (stages > kMaxStages) stages = kMaxStages;
-      while (na < 4 && (size_t)(na + 1) * p->a_slot_bytes + (size_t)stages * half <= budget) ++na;
-      p->na_slots = na;
-      p->stages = stages;
-      p->smem_bytes = fixed + (size_t)na * p->a_slot_bytes + (size_t)stages * half;
-      p->num_tiles = (p->num_m_tiles / 2) * p->num_n_tiles;          // work items per CTA pair
-      const int pairs = p->num_tiles < sms / 2 ? p->num_tiles : sms / 2;
-      p->grid = 2 * pairs;
-      return HF_OK;
-    }
-  } else {
-    const size_t stage_bytes = (size_t)128 * row_bytes + (size_t)n_tile * row_bytes;
-    int stages = (int)(budget / stage_bytes);
-    if (stages > kMaxStages) stages = kMaxStages;
-    HF_REQUIRE(stages >= 2, "conv: not enough shared memory for 2 stages");
-    p->stages = stages;
-    p->smem_bytes = fixed + stages * stage_bytes;
-    p->num_tiles = p->num_m_tiles * p->num_n_tiles;
-  }
+  const size_t stage_bytes = (size_t)128 * row_bytes + (size_t)n_tile * row_bytes;
+  int stages = (int)(budget / stage_bytes);
+  if (stages > kMaxStages) stages = kMaxStages;
+  HF_REQUIRE(stages >= 2, "conv: not enough shared memory for 2 stages");
+  p->stages = stages;
+  p->smem_bytes = fixed + stages * stage_bytes;
+  p->num_tiles = p->num_m_tiles * p->num_n_tiles;
   p->grid = p->num_tiles < sms ? p->num_tiles : sms;
   return HF_OK;
 }
 
-template <typename K>
-static int launch_kernel(K kern, int threads, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                         const ConvKernelParams& kp, const ConvPlan& pl, cudaStream_t st, const char* name) {
-  HF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-  kern<<<pl.grid, threads, pl.smem_bytes, st>>>(tmA, tmB, kp);
-  HF_LAUNCH_OK(name);
-  count_launch();
-  return HF_OK;
-}
-
-template <typename K>
-static int launch_pair_kernel(K kern, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvKernelParams& kp,
+template <int KCHUNK, int DT>
+static int launch_conv_kernel(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvKernelParams& kp,
                               const ConvPlan& pl, cudaStream_t st) {
-  HF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(pl.grid);
-  cfg.blockDim = dim3(kHaloThreads);
-  cfg.dynamicSmemBytes = pl.smem_bytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  HF_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, kp));
-  HF_LAUNCH_OK("conv_halo2");
+  void (*kern)(const CUtensorMap, const CUtensorMap, const ConvKernelParams) =
+      n_tile == 32 ? conv_wgmma_kernel<KCHUNK, DT, 32>
+                   : (n_tile == 64 ? conv_wgmma_kernel<KCHUNK, DT, 64> : conv_wgmma_kernel<KCHUNK, DT, 128>);
+  HF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+  kern<<<pl.grid, kConvThreads, pl.smem_bytes, st>>>(tmA, tmB, kp);
+  HF_LAUNCH_OK("conv_wgmma");
   count_launch();
   return HF_OK;
 }
@@ -1107,6 +605,7 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
   HF_REQUIRE(!a.noise || a.noise_w, "conv: noise given without noise weight");
   HF_REQUIRE((((uintptr_t)a.xhat_in | (uintptr_t)a.wpk | (uintptr_t)a.xhat_out) & 15) == 0,
              "conv: 16-bit tensors must be 16-byte aligned");
+  HF_REQUIRE(pl.n_tile == 32 || pl.n_tile == 64 || pl.n_tile == 128, "conv: N tile %d has no kernel", pl.n_tile);
 
   const int stride = a.stride ? a.stride : 1, groups = a.groups ? a.groups : 1;
   const int cin_g = a.Cin / groups;
@@ -1116,7 +615,6 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
     uint64_t strides[3] = {(uint64_t)a.Cin * 2, (uint64_t)a.W * a.Cin * 2, (uint64_t)a.H * a.W * a.Cin * 2};
     uint32_t box[4] = {(uint32_t)pl.kchunk, (uint32_t)pl.TW, (uint32_t)pl.TH, (uint32_t)pl.TB};
     uint32_t es[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
-    if (pl.halo) { box[1] = (uint32_t)pl.pitch; box[2] = kHaloRows; box[3] = 1; }
     // stride 2: the box is traversed with element stride 2, so it must span 2*T elements to deliver T samples
     if (stride == 2) { box[1] = (uint32_t)pl.TW * 2; box[2] = (uint32_t)pl.TH * 2; }
     rc = encode_tmap(&tmA, a.dtype, 4, const_cast<void*>(a.xhat_in), dims, strides, box, pl.kchunk * 2,
@@ -1128,12 +626,13 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
     const uint64_t N = a.up ? 4ull * a.Cout : (uint64_t)a.Cout;
     uint64_t dims[2] = {K, N};
     uint64_t strides[1] = {K * 2};
-    uint32_t box[2] = {(uint32_t)pl.kchunk, (uint32_t)(pl.halo == 2 ? 128 : pl.n_tile)};
+    uint32_t box[2] = {(uint32_t)pl.kchunk, (uint32_t)pl.n_tile};
     rc = encode_tmap(&tmB, a.dtype, 2, const_cast<void*>(a.wpk), dims, strides, box, pl.kchunk * 2);
     if (rc) return rc;
   }
 
   ConvKernelParams kp;
+  memset(&kp, 0, sizeof(kp));
   kp.B = a.B; kp.H = a.H; kp.W = a.W; kp.Cin = a.Cin; kp.Cout = a.Cout;
   kp.Ho = a.up ? 2 * a.H : (stride == 2 ? (a.H + 1) / 2 : a.H);
   kp.Wo = a.up ? 2 * a.W : (stride == 2 ? (a.W + 1) / 2 : a.W);
@@ -1146,9 +645,6 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
   kp.stages = pl.stages;
   kp.a_bytes = 128u * pl.kchunk * 2;
   kp.stage_bytes = kp.a_bytes + (uint32_t)pl.n_tile * pl.kchunk * 2;
-  kp.idesc = make_idesc_f16(a.dtype, pl.halo == 2 ? 256 : 128, pl.n_tile);
-  kp.G = pl.G; kp.na_slots = pl.na_slots; kp.pitch = pl.pitch; kp.b_resident = pl.b_resident;
-  kp.a_slot_bytes = pl.a_slot_bytes;
   kp.d = a.d;
   kp.noise = a.noise;
   kp.noise_bstride = (a.noise && a.noise_batch > 1) ? (int64_t)kp.Ho * kp.Wo : 0;
@@ -1160,7 +656,7 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
   kp.rgb_w = a.rgb_partial ? a.rgb_w : nullptr;
   kp.rgb_s = a.rgb_s;
   kp.rgb_partial = a.rgb_partial;
-  kp.dbg = env_int("HF_CONV_DBG", 0);       // experiments only: 1 = epilogue reduced to the TMEM read + release
+  kp.dbg = env_int("HF_CONV_DBG", 0);       // experiments only: 1 = epilogue reduced to the accumulator read
   kp.epi = a.epi; kp.stride = stride; kp.cin_g = cin_g; kp.enc_post = a.enc_post;
   kp.cout_g = (a.up ? 4 * a.Cout : a.Cout) / groups;
   kp.enc_act = a.enc_act; kp.enc_slope0 = a.enc_slope0;
@@ -1172,29 +668,11 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
   if (plan_out) *plan_out = pl;
 
   const bool bf = a.dtype == HF_BF16;
-  if (pl.halo == 2)
-    return bf ? launch_pair_kernel(conv_halo2_kernel<HF_BF16>, tmA, tmB, kp, pl, st)
-              : launch_pair_kernel(conv_halo2_kernel<HF_F16>, tmA, tmB, kp, pl, st);
-  if (pl.halo) {
-    constexpr int T4 = 64 + 128 * 4;
-    if (pl.ng == 4) {
-      if (pl.kchunk == 64)
-        return bf ? launch_kernel(conv_halo_kernel<64, HF_BF16, 4>, T4, tmA, tmB, kp, pl, st, "conv_halo")
-                  : launch_kernel(conv_halo_kernel<64, HF_F16, 4>, T4, tmA, tmB, kp, pl, st, "conv_halo");
-      return bf ? launch_kernel(conv_halo_kernel<32, HF_BF16, 4>, T4, tmA, tmB, kp, pl, st, "conv_halo")
-                : launch_kernel(conv_halo_kernel<32, HF_F16, 4>, T4, tmA, tmB, kp, pl, st, "conv_halo");
-    }
-    if (pl.kchunk == 64)
-      return bf ? launch_kernel(conv_halo_kernel<64, HF_BF16, 2>, kHaloThreads, tmA, tmB, kp, pl, st, "conv_halo")
-                : launch_kernel(conv_halo_kernel<64, HF_F16, 2>, kHaloThreads, tmA, tmB, kp, pl, st, "conv_halo");
-    return bf ? launch_kernel(conv_halo_kernel<32, HF_BF16, 2>, kHaloThreads, tmA, tmB, kp, pl, st, "conv_halo")
-              : launch_kernel(conv_halo_kernel<32, HF_F16, 2>, kHaloThreads, tmA, tmB, kp, pl, st, "conv_halo");
-  }
   if (pl.kchunk == 64)
-    return bf ? launch_kernel(conv_igemm_kernel<64, HF_BF16>, kConvThreads, tmA, tmB, kp, pl, st, "conv_igemm")
-              : launch_kernel(conv_igemm_kernel<64, HF_F16>, kConvThreads, tmA, tmB, kp, pl, st, "conv_igemm");
-  return bf ? launch_kernel(conv_igemm_kernel<32, HF_BF16>, kConvThreads, tmA, tmB, kp, pl, st, "conv_igemm")
-            : launch_kernel(conv_igemm_kernel<32, HF_F16>, kConvThreads, tmA, tmB, kp, pl, st, "conv_igemm");
+    return bf ? launch_conv_kernel<64, HF_BF16>(pl.n_tile, tmA, tmB, kp, pl, st)
+              : launch_conv_kernel<64, HF_F16>(pl.n_tile, tmA, tmB, kp, pl, st);
+  return bf ? launch_conv_kernel<32, HF_BF16>(pl.n_tile, tmA, tmB, kp, pl, st)
+            : launch_conv_kernel<32, HF_F16>(pl.n_tile, tmA, tmB, kp, pl, st);
 }
 
 }  // namespace hf

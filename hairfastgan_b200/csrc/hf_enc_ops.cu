@@ -1,4 +1,4 @@
-// Encoder-side kernels around the tcgen05 convolution (SURVEY 8 rows a13 / a14): plain-conv weight packing
+// Encoder-side kernels around the wgmma convolution (SURVEY 8 rows a13 / a14): plain-conv weight packing
 // (BatchNorm scale folded per output channel), NCHW fp32 <-> NHWC 16-bit conversion, squeeze-excite pooling
 // and combine, FPN bilinear upsample-add, adaptive average pooling.  All HBM-bound SIMT, fp32 math.
 #include <algorithm>
@@ -187,7 +187,7 @@ __global__ void __launch_bounds__(256) se_gate_kernel(const float* __restrict__ 
 
 int channel_reduce_splits(int B, int HW, int C) {
   const int64_t ctas = (int64_t)B * cdiv_i(C, 64);
-  int s = cdiv_i((int64_t)4 * 148, ctas);
+  int s = cdiv_i((int64_t)4 * num_sms(), ctas);
   s = std::min(s, std::max(1, HW / 64));
   return std::max(1, std::min(s, 64));
 }

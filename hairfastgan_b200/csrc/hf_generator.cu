@@ -1,4 +1,4 @@
-// Generator.forward (models/stylegan2/model.py:477-565) as one host-side chain of sm_100a kernels.
+// Generator.forward (models/stylegan2/model.py:477-565) as one host-side chain of sm_90a kernels.
 //
 // Per forward: 1 affine launch (all style modulations), 1 demod launch, 1 NCHW->NHWC pre-pass for the
 // first executed conv, then per layer {up-conv, conv, rgb_combine}.  Every conv epilogue applies

@@ -1,4 +1,4 @@
-// Internal launcher declarations shared by the translation units of libhairfast_sm100.so.
+// Internal launcher declarations shared by the translation units of libhairfast_sm90.so.
 #pragma once
 #include "hf_common.cuh"
 
@@ -93,7 +93,7 @@ int launch_adaptive_avgpool(const void* x16, float* y, int B, int H, int W, int 
                             cudaStream_t st);
 int ensure_device_current();
 
-// ---- hf_conv_tc.cu : tcgen05 implicit-GEMM convolution ----------------------------------------
+// ---- hf_conv_tc.cu : wgmma implicit-GEMM convolution ----------------------------------------
 struct ConvLaunch {
   int B, H, W;            // input spatial size
   int Cin, Cout;
@@ -132,11 +132,13 @@ struct ConvLaunch {
   void* enc_y16b;
 };
 struct ConvPlan {
-  int halo;               // 1: conv_halo_kernel (halo tile in smem, shifted descriptors); 0: conv_igemm_kernel
-  int G;                  // halo: tiles per round (share one accumulator buffer and each weight tile)
-  int ng;                 // halo: epilogue groups = TMEM accumulator buffers (2 x 256 or 4 x 128 columns)
-  int na_slots, pitch;    // halo: ring slots, halo row pitch in pixels
-  int b_resident;         // halo: whole weight matrix stays in smem
+  // halo, G, na_slots, pitch, b_resident, a_slot_bytes: halo-tile scheduling fields of the plan query ABI
+  // (hf_conv_plan_query); conv_wgmma_kernel loads one box per (tap, channel chunk) and reports 0 / 1 / 0 / 0 / 0 / 0.
+  int halo;
+  int G;
+  int ng;                 // consumer warpgroups (MMA + epilogue), 64 GEMM rows each
+  int na_slots, pitch;
+  int b_resident;
   uint32_t a_slot_bytes;
   int TW, TH, TB;         // pixel tile: TW*TH*TB = 128 GEMM rows
   int tiles_x, tiles_y, tiles_b, num_m_tiles;

@@ -1,4 +1,4 @@
-// Kernels around the tcgen05 convolution for the BiSeNet face-parsing network (SURVEY 8f-3; reference
+// Kernels around the wgmma convolution for the BiSeNet face-parsing network (SURVEY 8f-3; reference
 // models/CtrlHair/external_code/face_parsing/{model,resnet}.py): the 7x7 stride-2 RGB stem, 3x3 stride-2 max pooling,
 // pooled 1x1 "attention" convolutions, gated add with nearest 2x upsampling, and the final bilinear logit upsampling.
 // All SIMT, fp32 math, deterministic.
@@ -262,7 +262,7 @@ int launch_gate_add_up(const void* x16, const float* gate, const float* addvec, 
 // Roofline: 1.23 GFLOP against 3 MB in + 8.4 MB out per 512^2 image = 108 FLOP/B, far left of the ridge (~260): the
 // kernel is HBM-bound, so the contraction runs on warp-level mma.sync.m16n8k16 fragments built straight from a
 // shared-memory copy of the input window (K = 7 rows x 24 [= 7 taps x 3 channels + 3 zero-weight pads] = 168 -> 176);
-// a tcgen05 tile would need the same im2col rows materialised in the swizzled UMMA layout first.
+// a tensor-core tile would need the same im2col rows materialised in the swizzled operand layout first.
 // CTA = 8 x 32 output pixels x 64 channels, 8 warps (one output row each: 2 m16 tiles x 8 n8 tiles x 11 k16 steps).
 // ------------------------------------------------------------------------------------------------
 constexpr int kSfRows = 8, kSfCols = 32;                 // output tile
@@ -406,7 +406,7 @@ __global__ void __launch_bounds__(256, 2) stem7x7s2_fused_kernel(const float* __
 // (encoder4editing/models/encoders/psp_encoders.py:176-178 `input_layer`; FeatureStyleEncoder/arcface/iresnet.py:92-95
 // conv1/bn1/prelu as taken by nets/feature_style_encoder.py:27; models/Net.py:347) in ONE kernel: fp32 NCHW image in,
 // the raw 16-bit NHWC [B,H,W,64] activation AND its BatchNorm-affined copy for the first block out.  It replaces an
-// NCHW->NHWC(32) layout pass plus a tcgen05 convolution whose K = 9 x 32 was 90 % zero padding (Cin 3 -> 32).  Same
+// NCHW->NHWC(32) layout pass plus an implicit-GEMM convolution whose K = 9 x 32 was 90 % zero padding (Cin 3 -> 32).  Same
 // scheme as the 7x7 stem above (HBM-bound: 0.8 MB in, 16.8 MB out per 256^2 image): window gathered in shared memory
 // interleaved [row][x*4 + c] (c = 3 is a zero lane so that every k pair is one aligned 32-bit word), k = ky*16 + kx*4 + c
 // (K = 48), mma.sync fragments, persistent CTAs with the 7 KB of packed weights resident.

@@ -1,4 +1,4 @@
-"""e4e and FeatureStyleEncoder inversion encoders on the B200 convolution kernels (SURVEY 8 rows a13 / a14).
+"""e4e and FeatureStyleEncoder inversion encoders on the H100 convolution kernels (SURVEY 8 rows a13 / a14).
 
 Drop-in module surface (same class names, constructor arguments and ``state_dict`` keys, so the reference
 checkpoints load unchanged):
@@ -9,7 +9,7 @@ checkpoints load unchanged):
   -- models/FeatureStyleEncoder/nets/feature_style_encoder.py:12-65 and arcface/iresnet.py:28-163.
 
 The nn.Modules below only own parameters; ``forward`` runs NHWC 16-bit activations through
-``hf_conv2d_forward`` (tcgen05 implicit GEMM; eval-mode BatchNorm folded into weights / epilogue, PReLU /
+``hf_conv2d_forward`` (wgmma implicit GEMM; eval-mode BatchNorm folded into weights / epilogue, PReLU /
 LeakyReLU / residual add fused) plus a few HBM-bound glue kernels (``nn16``: SE pooling + gate, SE combine,
 FPN upsample-add, adaptive pooling).  The small dense style heads (EqualLinear / nn.Linear) are plain cuBLAS GEMMs
 through torch.

@@ -1,4 +1,4 @@
-"""B200-native StyleGAN2 generator modules -- a drop-in for the reference module surface
+"""H100-native StyleGAN2 generator modules -- a drop-in for the reference module surface
 ``models/stylegan2/model.py`` (PixelNorm :16, Upsample :35, Downsample :56, Blur :77, EqualLinear :134,
 ModulatedConv2d :183, NoiseInjection :282, ConstantInput :296, StyledConv :309, ToRGB :346,
 Generator :368): identical constructor / forward signatures and identical ``state_dict`` keys, so
@@ -6,7 +6,7 @@ Generator :368): identical constructor / forward signatures and identical ``stat
 in models/{Embedding,Alignment,Blending}.py work unchanged.
 
 The modules only hold parameters and translate the call into one C-ABI call of
-libhairfast_sm100.so (include/hairfast_b200.h):
+libhairfast_sm90.so (include/hairfast_b200.h):
 
 * ``Generator.forward``      -> ``hf_generator_forward`` (whole chain, fused epilogues)
 * ``StyledConv`` / ``ModulatedConv2d`` -> ``hf_conv_forward``

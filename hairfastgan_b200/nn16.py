@@ -1,5 +1,5 @@
-"""Thin Python layer over the encoder entry points of libhairfast_sm100.so (include/hairfast_b200.h,
-"Encoder backbones"): NHWC 16-bit activations, tcgen05 convolutions with folded BatchNorm / PReLU /
+"""Thin Python layer over the encoder entry points of libhairfast_sm90.so (include/hairfast_b200.h,
+"Encoder backbones"): NHWC 16-bit activations, wgmma convolutions with folded BatchNorm / PReLU /
 LeakyReLU / residual epilogues, and the HBM-bound glue kernels around them.  CUDA only, forward only."""
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""PostProcess conv stack of HairFast's Blending stage (SURVEY 8f-1) on the tcgen05 convolution kernels.
+"""PostProcess conv stack of HairFast's Blending stage (SURVEY 8f-1) on the wgmma convolution kernels.
 
 Drop-in counterparts of the reference classes ``PostProcessModel`` builds (models/Encoders.py:106-118):
 

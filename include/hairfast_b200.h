@@ -1,6 +1,6 @@
-/* hairfast_b200.h -- C ABI of libhairfast_sm100.so
+/* hairfast_b200.h -- C ABI of libhairfast_sm90.so
  *
- * B200 (sm_100a) implementation of the HairFastGAN hot path: the StyleGAN2 generator forward
+ * H100 (sm_90a) implementation of the HairFastGAN hot path: the StyleGAN2 generator forward
  * (ModulatedConv2d / StyledConv / ToRGB / upfirdn2d / fused bias+LeakyReLU).  Plain pointers and
  * sizes only -- no torch types.  All pointers are DEVICE pointers unless stated otherwise; every
  * output buffer is caller-allocated (the library never allocates device memory); every call
@@ -24,7 +24,7 @@ extern "C" {
 #define HF_OK 0
 #define HF_ERR_INVALID (-1)     /* bad argument / unsupported shape */
 #define HF_ERR_CUDA (-2)        /* CUDA runtime / driver error */
-#define HF_ERR_UNSUPPORTED (-3) /* device is not sm_100 */
+#define HF_ERR_UNSUPPORTED (-3) /* device is not sm_90 */
 
 /* 16-bit storage/operand type of the tensor-core path (accumulation is always fp32) */
 #define HF_BF16 0
@@ -113,7 +113,7 @@ int hf_conv_plan_query(const hf_conv_desc* d, int batch, int height, int width, 
 int hf_conv_forward(const hf_conv_desc* d, const void* packed, const hf_conv_io* io, void* stream);
 
 /* Measurement helper (no reference counterpart): runs hf_conv_forward's prologue once, then the
- * tcgen05 convolution kernel alone `iters` times between two CUDA events recorded on `stream`, and
+ * wgmma convolution kernel alone `iters` times between two CUDA events recorded on `stream`, and
  * returns the average kernel duration in milliseconds (host pointer).  Synchronises the stream. */
 int hf_conv_time_kernel(const hf_conv_desc* d, const void* packed, const hf_conv_io* io, int iters,
                         float* avg_ms /* host */, void* stream);

@@ -1,5 +1,5 @@
 """Generate the committed golden vectors under tests/golden/ by running the
-UNMODIFIED reference (imported from /root/reference, CPU fp32 branches) on
+UNMODIFIED reference (imported from the checkout named by HAIRFAST_REFERENCE, CPU fp32 branches) on
 seeded synthetic parameters.  Test infrastructure only (see oracle/README.md).
 
 Run once in the build container (the reference does not exist on the GPU box):
@@ -9,7 +9,7 @@ Run once in the build container (the reference does not exist on the GPU box):
 The reference's op package JIT-builds two CUDA extensions at import time
 (models/stylegan2/op/fused_act.py:10-16, upfirdn2d.py:10-16).  CPU tensors never
 touch them (fused_act.py:86, upfirdn2d.py:146), so ``cpp_extension.load`` is
-stubbed for this process; nothing in /root/reference is modified or copied.
+stubbed for this process; nothing in the checkout is modified or copied.
 """
 from __future__ import annotations
 
@@ -23,7 +23,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path.insert(0, ROOT)
 GOLD = os.path.join(ROOT, "tests", "golden")
-REF = os.environ.get("HAIRFAST_REFERENCE", "/root/reference")
+REF = os.environ["HAIRFAST_REFERENCE"]          # path of an unmodified reference checkout
 
 
 def import_reference():

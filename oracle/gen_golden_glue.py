@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path.insert(0, ROOT)
 GOLD = os.path.join(ROOT, "tests", "golden")
-REF = os.environ.get("HAIRFAST_REFERENCE", "/root/reference")
+REF = os.environ["HAIRFAST_REFERENCE"]          # path of an unmodified reference checkout
 
 
 def main():

@@ -23,12 +23,12 @@ def _run(*args, timeout=900, env=None):
 
 @pytest.mark.parametrize("arm", ["reference", "port"])
 def test_reference_arm_line(arm):
-    """`--impl reference`: the stock reference modules on the host cores when the checkout is staged (kind
+    """`--impl reference`: the stock reference modules on the host cores when the reference is built (kind
     "reference"), the oracle port otherwise (kind "port"); OMP_NUM_THREADS=1 as torchrun exports it must not shrink
     the thread count."""
     from baseline import refenv
     if arm == "reference" and not refenv.available():
-        pytest.skip("reference checkout not staged")
+        pytest.skip("reference not built (oracle/build_ref.py)")
     d = _run("--impl", "reference", "--steps", "1", "--warmup", "0", env={"HAIRFAST_CPU_ARM": arm,
                                                                           "OMP_NUM_THREADS": "1"})
     assert BASE_KEYS <= set(d) and d["impl"] == "reference"

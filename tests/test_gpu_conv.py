@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 ModulatedConv2d / StyledConv / ToRGB path (through hf_conv_forward /
+"""GPU parity of the wgmma ModulatedConv2d / StyledConv / ToRGB path (through hf_conv_forward /
 hf_torgb_forward) against the CPU oracle and the reference-generated golden vectors."""
 import os
 

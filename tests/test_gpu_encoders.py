@@ -1,5 +1,5 @@
 """GPU parity of the encoder rows (SURVEY 8 a13 / a14): the drop-in Encoder4Editing / fs_encoder_v2 modules
-(tcgen05 convs with folded BatchNorm / PReLU / SE / residual epilogues) against the reference-generated
+(wgmma convs with folded BatchNorm / PReLU / SE / residual epilogues) against the reference-generated
 golden vectors and the CPU oracle, plus the plain-conv building block against torch fp32."""
 import os
 import types

@@ -1,12 +1,11 @@
-"""The unmodified `HairFast(get_parser().parse_args([])).swap(face, shape, color)` of the staged reference checkout
+"""The unmodified `HairFast(get_parser().parse_args([])).swap(face, shape, color)` of the unmodified reference
 (hair_swap.py:27-105), end to end on the GPU, three ways: the stock reference (cuDNN + its JIT kernels), the same
 checkout under hairfastgan_b200.install(), and under install(skip_fse_reconstruction=True).  BASELINE configs[2] /
 SURVEY 8d config 3: three `torch.rand(3,1024,1024)` images (seeds 0,1,2), synthetic checkpoints
 (baseline/synth_checkpoints.py), default seed 3407.
 
 Each arm is its own process (the reference's modules are cached in sys.modules; one process = one mode).  The reference
-tree is staged by tools/stage_reference.sh into baseline/_ref (git-ignored, travels with the gpurun snapshot); the test
-skips when it is absent.
+is what oracle/build_ref.py built under oracle/_ref (git-ignored); the test skips when it is absent.
 """
 import json
 import os
@@ -20,7 +19,7 @@ from baseline import refenv
 from tests.gpu_util import ROOT, record
 
 pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not refenv.available(), reason="reference not staged (tools/stage_reference.sh)")]
+              pytest.mark.skipif(not refenv.available(), reason="reference not built (oracle/build_ref.py)")]
 
 WORK = os.environ.get("HAIRFAST_WORK", "/tmp/hairfast_work")
 # "default" = nothing set in the environment: generator bf16, encoder family fp16 (what a user of install() gets)
@@ -31,8 +30,6 @@ HF_DTYPES = os.environ.get("HAIRFAST_SWAP_DTYPES", "default").split(",")
 # seeds.  The pipeline has discrete decisions (BiSeNet arg-max labels -> 256^2 masks -> F-space blends), so a small set
 # of pixels near label boundaries can move by more than the arithmetic error; the bound is therefore on the mean and on
 # a high quantile, with the max reported.
-# Measured on B200 (round 2), mean / q99 / max: all-bf16 1.7e-4 / 5.8e-4 / 1.6e-3; default (generator bf16, encoders
-# fp16) 9.6e-5 / 3.3e-4 / 8.5e-4; all-fp16 3.0e-5 / 1.2e-4 / 4.0e-4.  Stated bounds = ~4x the measurement.
 TOL_FINAL_MEAN = {"default": 4e-4, "bf16": 8e-4, "fp16": 1.5e-4}
 TOL_FINAL_Q99 = {"default": 1.5e-3, "bf16": 2.5e-3, "fp16": 5e-4}
 TOL_FINAL_MAX = {"default": 5e-3, "bf16": 8e-3, "fp16": 2e-3}

@@ -1,4 +1,4 @@
-"""Build-container check (skipped where the reference checkout is absent, e.g. on the GPU box): with
+"""Check against the reference built by oracle/build_ref.py (skipped where it was not built): with
 ``hairfastgan_b200.install.install()`` active, the UNMODIFIED reference modules that swap() imports resolve the hot-path
 classes to this package.  Third-party packages the image lacks (dlib, clip, lpips, ...) are replaced by inert stubs;
 nothing is constructed or run -- this is about import-time name resolution only.  Runs in a fresh interpreter."""
@@ -10,7 +10,10 @@ import textwrap
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("HAIRFAST_REFERENCE", "/root/reference")
+sys.path.insert(0, ROOT)
+from baseline import refenv  # noqa: E402
+
+REF = refenv.REF_ROOT
 
 PROBE = textwrap.dedent("""
     import importlib, sys, types
@@ -82,7 +85,7 @@ EXPECTED = {
 }
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "models")), reason="reference checkout not present")
+@pytest.mark.skipif(not refenv.available(), reason="reference not built (oracle/build_ref.py)")
 def test_reference_imports_resolve_to_this_package(tmp_path):
     p = subprocess.run([sys.executable, "-c", PROBE % {"root": ROOT, "ref": REF}], capture_output=True, text=True,
                        timeout=600, cwd=str(tmp_path))

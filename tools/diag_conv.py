@@ -1,4 +1,4 @@
-"""GPU bring-up diagnostics for the tcgen05 conv kernel: runs a ladder of ModulatedConv2d cases from
+"""GPU bring-up diagnostics for the wgmma conv kernel: runs a ladder of ModulatedConv2d cases from
 a bare 1x1 GEMM to the full fused StyledConv and prints where (which channel group / pixel rows) the
 result departs from the CPU oracle.  Writes gpurun_out/diag.txt.  Test infrastructure."""
 import os
