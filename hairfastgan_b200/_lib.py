@@ -115,7 +115,6 @@ SYMBOLS = {
     "hf_stem3x3_nhwc16": (C.c_int, [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "hf_stem7x7s2_nhwc16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                       C.c_void_p]),
-    "hf_im2col7x7s2_nhwc16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "hf_maxpool3x3s2_nhwc16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                          C.c_void_p]),
     "hf_pooled_fc_nhwc16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,

@@ -140,12 +140,6 @@ int hf_stem3x3_nhwc16(const float* x, const void* wpacked, const float* shift, c
                               (cudaStream_t)stream);
 }
 
-int hf_im2col7x7s2_nhwc16(const float* x, void* y16, int batch, int height, int width, int dtype, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  return launch_im2col7x7s2(x, y16, batch, height, width, dtype, (cudaStream_t)stream);
-}
-
 int hf_maxpool3x3s2_nhwc16(const void* x16, void* y16, int batch, int height, int width, int channels, int dtype,
                            void* stream) {
   int rc = ensure_device_current();

@@ -61,7 +61,6 @@ int launch_nhwc16_to_nchw(const void* x16, float* y, int B, int C, int HW, int d
 int channel_reduce_splits(int B, int HW, int C);
 int launch_channel_partial(const void* x16, float* ws, int B, int HW, int C, int dtype, cudaStream_t st, int* splits);
 // BiSeNet glue (hf_seg_ops.cu)
-int launch_im2col7x7s2(const float* x, void* y16, int B, int H, int W, int dtype, cudaStream_t st);
 int launch_stem7x7s2_fused(const float* x, const void* wpacked, const float* shift, void* y16, int B, int H, int W,
                            int dtype, cudaStream_t st);
 int launch_stem3x3_fused(const float* x, const void* wpacked, const float* shift, const float* slope, const float* s2,

@@ -13,289 +13,18 @@ static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 //             op/upfirdn2d_kernel.cu:107-207 -- zero-stuff, pad/crop, convolve (flipped taps), decimate)
 // =============================================================================================
 
-// Fast path: up = 1, 4x4 taps, down in {1,2}.  One CTA = one (plane, 32x64 | 16x64 output tile);
-// the input window is staged once in shared memory with coalesced row loads, each thread produces
-// 4 consecutive outputs per row from a sliding register window and stores them as one float4.
-template <int DOWN, int ROWS>
-__global__ void __launch_bounds__(256) upfirdn2d_up1_k4_kernel(const float* __restrict__ x, float* __restrict__ y,
-                                                               const float* __restrict__ k, int in_h, int in_w,
-                                                               int out_h, int out_w, int px0, int py0) {
-  constexpr int TW = 64;
-  constexpr int IN_ROWS = (ROWS - 1) * DOWN + 4;
-  constexpr int IN_COLS = (TW - 1) * DOWN + 4;
-  constexpr int PITCH = (IN_COLS + 3) / 4 * 4;          // rows start 16-byte aligned: the window is read as float4
-  __shared__ __align__(16) float tile[IN_ROWS * PITCH];
-  __shared__ float kf[16];
-  const int plane = blockIdx.z;
-  const int oy0 = blockIdx.y * ROWS, ox0 = blockIdx.x * TW;
-  const float* xp = x + (size_t)plane * in_h * in_w;
-  if (threadIdx.x < 16) kf[threadIdx.x] = k[15 - threadIdx.x];   // flipped: kf[ky][kx] = k[3-ky][3-kx]
-  const int gy0 = oy0 * DOWN - py0, gx0 = ox0 * DOWN - px0;
-  // staging in two unrolled phases -- all global loads of a thread are issued before the first shared store, so
-  // their latencies overlap (a rolled load->store loop paid one HBM round trip per element: 0.29 of the copy peak)
-  constexpr int N_STAGE = (IN_ROWS * IN_COLS + 255) / 256;
-  float stage[N_STAGE];
-#pragma unroll
-  for (int it = 0; it < N_STAGE; ++it) {
-    const int i = threadIdx.x + it * 256;
-    const int r = i / IN_COLS, c = i - r * IN_COLS;
-    const int gy = gy0 + r, gx = gx0 + c;
-    stage[it] = (i < IN_ROWS * IN_COLS && gy >= 0 && gy < in_h && gx >= 0 && gx < in_w)
-                    ? __ldg(xp + (size_t)gy * in_w + gx) : 0.f;
-  }
-#pragma unroll
-  for (int it = 0; it < N_STAGE; ++it) {
-    const int i = threadIdx.x + it * 256;
-    if (i < IN_ROWS * IN_COLS) {
-      const int r = i / IN_COLS, c = i - r * IN_COLS;
-      tile[r * PITCH + c] = stage[it];
-    }
-  }
-  __syncthreads();
-  float kr[16];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) kr[i] = kf[i];
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;   // 16 x 16 threads
-  float* yp = y + (size_t)plane * out_h * out_w;
-#pragma unroll
-  for (int rr = 0; rr < ROWS / 16; ++rr) {
-    const int r = ty + rr * 16;
-    const int oy = oy0 + r, ox = ox0 + tx * 4;
-    float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int ky = 0; ky < 4; ++ky) {
-      const float4* row4 = reinterpret_cast<const float4*>(tile + (r * DOWN + ky) * PITCH + tx * 4 * DOWN);
-      constexpr int NW4 = (3 * DOWN + 4 + 3) / 4;
-      float w[NW4 * 4];
-#pragma unroll
-      for (int i = 0; i < NW4; ++i) {
-        const float4 t4 = row4[i];
-        w[4 * i] = t4.x; w[4 * i + 1] = t4.y; w[4 * i + 2] = t4.z; w[4 * i + 3] = t4.w;
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-#pragma unroll
-        for (int kx = 0; kx < 4; ++kx) acc[j] = fmaf(w[j * DOWN + kx], kr[ky * 4 + kx], acc[j]);
-    }
-    if (oy < out_h) {
-      float* dst = yp + (size_t)oy * out_w + ox;
-      if (ox + 3 < out_w && ((out_w & 3) == 0)) {
-        *reinterpret_cast<float4*>(dst) = make_float4(acc[0], acc[1], acc[2], acc[3]);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (ox + j < out_w) dst[j] = acc[j];
-      }
-    }
-  }
-}
-
-// Fast path: up = 2, down = 1, 4x4 taps (the RGB-skip Upsample, model.py:35-53).  Only 2x2 of the
-// 16 taps hit a non-zero sample; each thread makes 4 consecutive outputs of one row.  (A row-per-CTA variant with
-// the two live input rows staged in shared memory measured slower: 1.06 vs 1.41 TB/s.)
-__global__ void __launch_bounds__(256) upfirdn2d_up2_k4_kernel(const float* __restrict__ x, float* __restrict__ y,
-                                                               const float* __restrict__ k, int in_h, int in_w,
-                                                               int out_h, int out_w, int px0, int py0,
-                                                               int64_t total_quads) {
-  __shared__ float kf[16];
-  if (threadIdx.x < 16) kf[threadIdx.x] = k[15 - threadIdx.x];
-  __syncthreads();
-  const int quads_per_row = (out_w + 3) >> 2;
-  // 32-bit index math (the launcher checks total_quads < 2^31)
-  for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < (int)total_quads; q += gridDim.x * blockDim.x) {
-    int qx = q % quads_per_row;
-    int t = q / quads_per_row;
-    int oy = t % out_h;
-    int plane = t / out_h;
-    const float* xp = x + (size_t)plane * in_h * in_w;
-    const int ky0 = (py0 - oy) & 1;          // oy + ky - py0 must be even
-    float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int a = 0; a < 2; ++a) {
-      const int ky = ky0 + 2 * a;
-      const int uy = oy + ky - py0;
-      const int iy = uy >> 1;
-      if (uy < 0 || iy >= in_h) continue;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int ox = qx * 4 + j;
-        const int kx0 = (px0 - ox) & 1;
-#pragma unroll
-        for (int b = 0; b < 2; ++b) {
-          const int kx = kx0 + 2 * b;
-          const int ux = ox + kx - px0;
-          const int ix = ux >> 1;
-          if (ux >= 0 && ix < in_w) acc[j] = fmaf(__ldg(xp + (size_t)iy * in_w + ix), kf[ky * 4 + kx], acc[j]);
-        }
-      }
-    }
-    float* dst = y + ((size_t)plane * out_h + oy) * out_w + qx * 4;
-    if ((out_w & 3) == 0) {
-      *reinterpret_cast<float4*>(dst) = make_float4(acc[0], acc[1], acc[2], acc[3]);
-    } else {
-      for (int j = 0; j < 4; ++j)
-        if (qx * 4 + j < out_w) dst[j] = acc[j];
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Round-2 fast paths: register sliding windows, no shared memory, no block-level synchronisation.
-// A warp owns a strip of RS rows x 128 columns and walks down it; every lane keeps its 4 (or 2x8) outputs' partial
-// sums in registers and each input row is fetched ONCE per strip (plus the 3 / 2 halo rows, which the neighbouring
-// strip of the same CTA has just pulled into L1/L2).  All global accesses of a warp are row-contiguous (512 B per
-// row); the 4x4 FIR costs 64 FMAs per float4 of output, well under the issue budget of an HBM-bound kernel.
-// ---------------------------------------------------------------------------------------------
-// up = 1, down = 1, 4x4 taps, any pad >= 0 (the Blur after the transposed convolution, model.py:77-93).
-// Input side (round 2, after ncu: the register-window loads left every warp with ~1 row in flight -- long-scoreboard
-// stalls 15 per issue, 0.65 of the copy peak): each warp owns a ring of kUpStages row segments in shared memory and
-// keeps kUpStages - 1 rows AHEAD in flight with 4-byte cp.async (the (2R+1)-wide rows are only 4-byte aligned, so
-// neither 16-byte cp.async nor TMA applies): lane l copies elements l, l+32, ... of the 131-float segment, fully
-// coalesced, zero-filled outside the image (= the padding).  No block-level synchronisation: a warp only waits for
-// its own copy groups.
-constexpr int kUpStages = 8;                                 // power of two: slot = row & 7
-constexpr int kUpSeg = 136;                                  // 128 + 3 taps, padded to a multiple of 8 floats
-
-__device__ __forceinline__ void cp_async4_zfill(uint32_t dst_s, const float* src, bool pred) {
-  const int sz = pred ? 4 : 0;                               // src-size 0: the 4 destination bytes are zero-filled
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst_s), "l"(src), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-template <int RS>
-__global__ void __launch_bounds__(256) upfirdn2d_up1_k4_strip_kernel(const float* __restrict__ x,
-                                                                     float* __restrict__ y,
-                                                                     const float* __restrict__ k, int in_h, int in_w,
-                                                                     int out_h, int out_w, int px0, int py0, int wx) {
-  // wx (1, 2, 4 or 8) warps of a CTA sit SIDE BY SIDE (wx x 128 columns, up to a whole 1024-wide row) and walk down the
-  // same RS rows; the other 8 / wx warp groups take the strips below
-  __shared__ __align__(16) float ring[8][kUpStages][kUpSeg];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int oxw = (blockIdx.x * wx + (warp & (wx - 1))) * 128;       // first output column of this warp
-  const int ox = oxw + lane * 4;
-  const int oy0 = (blockIdx.y * (8 / wx) + warp / wx) * RS;
-  if (oy0 >= out_h || oxw >= out_w) return;                           // whole warps only: the ring is per warp
-  float kr[16];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) kr[i] = __ldg(k + 15 - i);           // flipped taps: kr[a*4+b] = k[3-a][3-b]
-  // rank-1 test on the flipped taps: kr[a][b] == ky[a] * kx[b] with kx = row 0, ky = column 0 / kr[0][0]
-  float kx[4], ky[4];
-  bool separable = kr[0] != 0.f;
-#pragma unroll
-  for (int b = 0; b < 4; ++b) kx[b] = kr[b];
-#pragma unroll
-  for (int a = 0; a < 4; ++a) ky[a] = separable ? kr[a * 4] / kr[0] : 0.f;
-#pragma unroll
-  for (int a = 0; a < 4; ++a)
-#pragma unroll
-    for (int b = 0; b < 4; ++b)
-      separable = separable && fabsf(ky[a] * kx[b] - kr[a * 4 + b]) <= 1e-6f * fabsf(kr[a * 4 + b]) + 1e-30f;
-  const float* xp = x + (size_t)blockIdx.z * in_h * in_w;
-  float* yp = y + (size_t)blockIdx.z * out_h * out_w;
-  const int ixw = oxw - px0;                                          // first input column of the warp's segment
-  const bool vec_store = ((out_w & 3) == 0) && ox + 3 < out_w;
-  const uint32_t ring_s = (uint32_t)__cvta_generic_to_shared(&ring[warp][0][0]);
-  constexpr int NROWS = RS + 3;
-  // row r of the strip (input row iy = oy0 - py0 + r) -> ring slot r & (kUpStages - 1).  The column part of every
-  // copy (offset, in-bounds flag, shared address) is row-invariant and computed once
-  int gxo[5];
-  uint32_t dsto[5];
-  bool okx[5];
-#pragma unroll
-  for (int j = 0; j < 5; ++j) {
-    const int e = j * 32 + lane, gx = ixw + e;
-    okx[j] = e < 131 && gx >= 0 && gx < in_w;
-    gxo[j] = okx[j] ? gx : 0;
-    dsto[j] = ring_s + (uint32_t)(e < 131 ? e : 0) * 4u;
-  }
-  auto issue_row = [&](int r) {
-    const int iy = oy0 - py0 + r;
-    const bool row_ok = r < NROWS && iy >= 0 && iy < in_h;
-    const float* rp = xp + (size_t)(row_ok ? iy : 0) * in_w;
-    const uint32_t slot_off = (uint32_t)((r & (kUpStages - 1)) * kUpSeg) * 4u;
-#pragma unroll
-    for (int j = 0; j < 5; ++j)
-      if (j < 4 || lane < 3)                                          // element 128 + lane exists for lanes 0..2 only
-        cp_async4_zfill(dsto[j] + slot_off, rp + gxo[j], row_ok && okx[j]);
-    cp_async_commit();
-  };
-#pragma unroll
-  for (int r = 0; r < kUpStages - 1; ++r) issue_row(r);
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-#pragma unroll 1
-  for (int r0 = 0; r0 < NROWS; r0 += 4) {
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int r = r0 + u;
-      issue_row(r + kUpStages - 1);                                   // always commits a (possibly empty) group
-      cp_async_wait<kUpStages - 1>();                                 // row r has landed (this lane's copies) ...
-      __syncwarp();                                                   // ... and every other lane's
-      const float* seg = &ring[warp][r & (kUpStages - 1)][lane * 4];
-      const float4 s0 = *reinterpret_cast<const float4*>(seg);
-      const float4 s1 = *reinterpret_cast<const float4*>(seg + 4);
-      const float v[7] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z};
-      __syncwarp();                                                   // slot may be refilled by the next issue_row
-      // input row r feeds output rows r - a (a = tap row); (r - a) & 3 == (u - a) & 3 because r0 % 4 == 0
-      if (separable) {
-        // rank-1 FIR (every make_kernel() blur: outer(k1, k1)): one horizontal pass per input row, then 4 scaled adds
-        float hrow[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float t = v[j] * kx[0];
-#pragma unroll
-          for (int b = 1; b < 4; ++b) t = fmaf(v[j + b], kx[b], t);
-          hrow[j] = t;
-        }
-#pragma unroll
-        for (int a = 0; a < 4; ++a)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) acc[(u - a) & 3][j] = fmaf(hrow[j], ky[a], acc[(u - a) & 3][j]);
-      } else {
-#pragma unroll
-        for (int a = 0; a < 4; ++a)
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-#pragma unroll
-            for (int b = 0; b < 4; ++b) acc[(u - a) & 3][j] = fmaf(v[j + b], kr[a * 4 + b], acc[(u - a) & 3][j]);
-      }
-      const int orow = r - 3;                                        // complete once its a = 3 row has arrived
-      const int slot = (u + 1) & 3;
-      if (orow >= 0 && orow < RS && oy0 + orow < out_h && ox < out_w) {
-        float* dst = yp + (size_t)(oy0 + orow) * out_w + ox;
-        if (vec_store) {
-          __stcs(reinterpret_cast<float4*>(dst), make_float4(acc[slot][0], acc[slot][1], acc[slot][2], acc[slot][3]));
-        } else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (ox + j < out_w) dst[j] = acc[slot][j];
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j) acc[slot][j] = 0.f;
-    }
-  }
-  cp_async_wait<0>();
-}
-
 // up = 1, down in {1, 2}, 4x4 taps, pads 0..3, planes up to 1040 columns wide: the input side done by the TMA engine.
-// A strip of full-width rows of one plane is ONE contiguous span of global memory, so although its rows are only
-// 4-byte aligned (width 2R+1 after the transposed convolution) the span can be fetched with 1-D bulk copies
-// (`cp.async.bulk`, 16-byte aligned start and size: the span is widened to the enclosing 16-byte boundaries, which
-// stay inside the tensor because the launch checks base alignment and total size).  One elected thread keeps up to
-// S chunks of CR rows in flight per CTA (mbarrier complete_tx); there are no per-element copy instructions and no
-// per-element address arithmetic -- the cp.async ring above spends 36 instructions per output on that, this kernel
-// ~14 -- and the small stages (3 x 16 KB at 1025 columns) leave room for 4 CTAs per SM, which is what the HBM rate
-// turned out to depend on (measured on the [256,1025,1025] blur: 8-row chunks x 3, 2 CTAs/SM 5.0 TB/s; 4-row chunks
-// x 3, 4 CTAs/SM 6.1 TB/s = 0.93 of the copy peak; ring kernel 4.45).  A thread owns the output columns t, t+256, ...
-// (conflict-free 4-byte LDS whatever the row's alignment; 2-way for down = 2) and walks down the strip with the
-// separable (or general) FIR in registers exactly like the ring kernels; padding columns are handled by a masked path
-// that only the threads owning an edge column take, padding rows contribute nothing and are never fetched.
+// Rows are only 4-byte aligned (width 2R+1 after the transposed convolution), so neither 16-byte per-row copies nor a
+// tiled tensor map apply.  But a strip of full-width rows of one plane is ONE contiguous span of global memory, so it
+// is fetched with 1-D bulk copies (`cp.async.bulk`) of whole-row spans.  A bulk copy needs a 16-byte aligned start and
+// size, so the span is widened to the enclosing 16-byte boundaries; the widened span stays inside the tensor only
+// because the launcher checks that the base is 16-byte aligned and the total element count a multiple of 4.
+// One elected thread keeps up to S chunks of CR rows in flight per CTA (mbarrier complete_tx), so there are no
+// per-element copy instructions and no per-element address arithmetic.  The stages are kept small (3 x 16 KB at 1025
+// columns) so that several CTAs stay resident per SM and keep enough bytes in flight.  A thread owns the output
+// columns t, t+256, ... (conflict-free 4-byte LDS whatever the row's alignment; 2-way for down = 2) and walks down the
+// strip with the separable (or general) FIR in registers; padding columns are handled by a masked path that only the
+// threads owning an edge column take, padding rows contribute nothing and are never fetched.
 __device__ __forceinline__ void bulk_load_1d(uint32_t dst_s, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst_s), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
@@ -339,7 +68,8 @@ __global__ void __launch_bounds__(256) upfirdn2d_k4_bulk_kernel(const float* __r
 #pragma unroll
   for (int i = 0; i < 16; ++i) kr[i] = __ldg(k + 15 - i);           // flipped taps: kr[a*4+b] = k[3-a][3-b]
   float kx[4], ky[4];
-  bool separable = kr[0] != 0.f;                                      // rank-1 test, as in the ring kernels
+  // rank-1 test on the flipped taps: kr[a][b] == ky[a] * kx[b] with kx = row 0, ky = column 0 / kr[0][0]
+  bool separable = kr[0] != 0.f;
 #pragma unroll
   for (int b = 0; b < 4; ++b) kx[b] = kr[b];
 #pragma unroll
@@ -607,201 +337,6 @@ __global__ void __launch_bounds__(256) upfirdn2d_up2_k4_bulk_kernel(const float*
   }
 }
 
-// up = 1, down = 2, 4x4 taps, pad >= 0 (the Downsample / ConvLayer blur of the reference, model.py:56-74; not on the
-// swap path): same scheme as the up1 kernel -- per-warp cp.async ring, register accumulators -- with two input rows
-// and 2 x 128 + 2 input columns per output row.  Input row r = 2m + e feeds output row m with tap row e and output
-// row m - 1 with tap row e + 2, so two accumulator rows are live.
-constexpr int kDnStages = 4;
-constexpr int kDnSeg = 264;                                  // 258 floats per row segment, padded
-
-template <int RS>
-__global__ void __launch_bounds__(256) upfirdn2d_down2_k4_strip_kernel(const float* __restrict__ x,
-                                                                       float* __restrict__ y,
-                                                                       const float* __restrict__ k, int in_h, int in_w,
-                                                                       int out_h, int out_w, int px0, int py0) {
-  __shared__ __align__(16) float ring[8][kDnStages][kDnSeg];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int oxw = blockIdx.x * 128;
-  const int ox = oxw + lane * 4;
-  const int oy0 = (blockIdx.y * 8 + warp) * RS;
-  if (oy0 >= out_h) return;                                           // whole warps only: the ring is per warp
-  float kr[16];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) kr[i] = __ldg(k + 15 - i);           // flipped taps: kr[a*4+b] = k[3-a][3-b]
-  float kx[4], ky[4];
-  bool separable = kr[0] != 0.f;
-#pragma unroll
-  for (int b = 0; b < 4; ++b) kx[b] = kr[b];
-#pragma unroll
-  for (int a = 0; a < 4; ++a) ky[a] = separable ? kr[a * 4] / kr[0] : 0.f;
-#pragma unroll
-  for (int a = 0; a < 4; ++a)
-#pragma unroll
-    for (int b = 0; b < 4; ++b)
-      separable = separable && fabsf(ky[a] * kx[b] - kr[a * 4 + b]) <= 1e-6f * fabsf(kr[a * 4 + b]) + 1e-30f;
-  const float* xp = x + (size_t)blockIdx.z * in_h * in_w;
-  float* yp = y + (size_t)blockIdx.z * out_h * out_w;
-  const int ixw = 2 * oxw - px0;                                      // first input column of the warp's segment
-  const int iy_first = 2 * oy0 - py0;                                 // input row of strip row 0
-  const bool vec_store = ((out_w & 3) == 0) && ox + 3 < out_w;
-  const uint32_t ring_s = (uint32_t)__cvta_generic_to_shared(&ring[warp][0][0]);
-  constexpr int NROWS = 2 * RS + 2;
-  int gxo[9];
-  bool okx[9];
-#pragma unroll
-  for (int j = 0; j < 9; ++j) {
-    const int e = j * 32 + lane, gx = ixw + e;
-    okx[j] = e < 258 && gx >= 0 && gx < in_w;
-    gxo[j] = okx[j] ? gx : 0;
-  }
-  auto issue_row = [&](int r) {
-    const int iy = iy_first + r;
-    const bool row_ok = r < NROWS && iy >= 0 && iy < in_h;
-    const float* rp = xp + (size_t)(row_ok ? iy : 0) * in_w;
-    const uint32_t dst = ring_s + (uint32_t)((r & (kDnStages - 1)) * kDnSeg + lane) * 4u;
-#pragma unroll
-    for (int j = 0; j < 9; ++j)
-      if (j < 8 || lane < 2)                                          // elements 256, 257 exist for lanes 0, 1 only
-        cp_async4_zfill(dst + (uint32_t)(j * 32) * 4u, rp + gxo[j], row_ok && okx[j]);
-    cp_async_commit();
-  };
-#pragma unroll
-  for (int r = 0; r < kDnStages - 1; ++r) issue_row(r);
-  float acc[2][4];
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-#pragma unroll 1
-  for (int r0 = 0; r0 < NROWS; r0 += 4) {
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int r = r0 + u;                                           // r = 2m + e with m = r0/2 + (u >> 1), e = u & 1
-      issue_row(r + kDnStages - 1);
-      cp_async_wait<kDnStages - 1>();
-      __syncwarp();
-      const float* seg = &ring[warp][r & (kDnStages - 1)][lane * 8];
-      const float4 s0 = *reinterpret_cast<const float4*>(seg);
-      const float4 s1 = *reinterpret_cast<const float4*>(seg + 4);
-      const float4 s2 = *reinterpret_cast<const float4*>(seg + 8);
-      const float v[10] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w, s2.x, s2.y};
-      __syncwarp();
-      const int e = u & 1, cur = (u >> 1) & 1, prev = cur ^ 1;       // output m -> slot cur, output m - 1 -> slot prev
-      if (separable) {
-        float hrow[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float t = v[2 * j] * kx[0];
-#pragma unroll
-          for (int b = 1; b < 4; ++b) t = fmaf(v[2 * j + b], kx[b], t);
-          hrow[j] = t;
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          acc[cur][j] = fmaf(hrow[j], ky[e], acc[cur][j]);
-          acc[prev][j] = fmaf(hrow[j], ky[e + 2], acc[prev][j]);
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-#pragma unroll
-          for (int b = 0; b < 4; ++b) {
-            acc[cur][j] = fmaf(v[2 * j + b], kr[e * 4 + b], acc[cur][j]);
-            acc[prev][j] = fmaf(v[2 * j + b], kr[(e + 2) * 4 + b], acc[prev][j]);
-          }
-      }
-      if (e == 1) {                                                   // rows 2m-2 .. 2m+1 seen: output m - 1 is complete
-        const int orow = (r >> 1) - 1;
-        if (orow >= 0 && orow < RS && oy0 + orow < out_h && ox < out_w) {
-          float* dst = yp + (size_t)(oy0 + orow) * out_w + ox;
-          if (vec_store) {
-            __stcs(reinterpret_cast<float4*>(dst), make_float4(acc[prev][0], acc[prev][1], acc[prev][2], acc[prev][3]));
-          } else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              if (ox + j < out_w) dst[j] = acc[prev][j];
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[prev][j] = 0.f;
-      }
-    }
-  }
-  cp_async_wait<0>();
-}
-
-// up = 2, down = 1, 4x4 taps, pad (2,1): the RGB-skip Upsample (model.py:35-53), out = 2 x in.  Output parity (py,px)
-// has 2x2 live taps: out[2y+py][2x+px] = sum_{a,b in {0,1}} in[y-1+py+a][x-1+px+b] * kf[py+2a][px+2b].
-// A lane owns 4 input columns (8 output columns, two float4 stores per output row) and slides a 3-row window.
-template <int RS>
-__global__ void __launch_bounds__(256) upfirdn2d_up2_k4_strip_kernel(const float* __restrict__ x,
-                                                                     float* __restrict__ y,
-                                                                     const float* __restrict__ k, int in_h, int in_w,
-                                                                     int wx) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int x0 = (blockIdx.x * wx + (warp & (wx - 1))) * 128 + lane * 4;   // wx warps side by side (see the up1 kernel)
-  const int y0 = (blockIdx.y * (8 / wx) + warp / wx) * RS;
-  if (y0 >= in_h || x0 >= in_w) return;
-  float kr[16];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) kr[i] = __ldg(k + 15 - i);
-  const float* xp = x + (size_t)blockIdx.z * in_h * in_w;
-  const int out_w = 2 * in_w;
-  float* yp = y + (size_t)blockIdx.z * (2 * in_h) * out_w;
-  const bool interior = x0 >= 1 && x0 + 4 < in_w;
-  const bool full = x0 + 3 < in_w && (in_w & 1) == 0;               // 2*in_w % 4 == 0 and all 8 outputs exist
-  float win[3][6];
-  auto load_row = [&](int iy, float* v) {
-    const bool row_ok = iy >= 0 && iy < in_h;
-    const float* rp = xp + (size_t)(row_ok ? iy : 0) * in_w + x0 - 1;
-    if (row_ok && interior) {
-#pragma unroll
-      for (int c = 0; c < 6; ++c) v[c] = __ldg(rp + c);
-    } else {
-#pragma unroll
-      for (int c = 0; c < 6; ++c) v[c] = (row_ok && x0 - 1 + c >= 0 && x0 - 1 + c < in_w) ? __ldg(rp + c) : 0.f;
-    }
-  };
-  load_row(y0 - 1, win[0]);
-  load_row(y0, win[1]);
-#pragma unroll 1
-  for (int r0 = 0; r0 < RS; r0 += 3) {
-#pragma unroll
-    for (int u = 0; u < 3; ++u) {
-      const int yy = y0 + r0 + u;
-      // rows yy-1, yy, yy+1 live in slots u % 3, (u+1) % 3, (u+2) % 3
-      load_row((r0 + u < RS && yy < in_h) ? yy + 1 : -1, win[(u + 2) % 3]);
-      if (r0 + u < RS && yy < in_h) {
-#pragma unroll
-        for (int py = 0; py < 2; ++py) {
-          float o[8];
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int px = 0; px < 2; ++px) {
-              float s = 0.f;
-#pragma unroll
-              for (int a = 0; a < 2; ++a)
-#pragma unroll
-                for (int b = 0; b < 2; ++b)
-                  s = fmaf(win[(u + py + a) % 3][i + px + b], kr[(py + 2 * a) * 4 + px + 2 * b], s);
-              o[2 * i + px] = s;
-            }
-          float* dst = yp + (size_t)(2 * yy + py) * out_w + 2 * x0;
-          if (full) {
-            __stcs(reinterpret_cast<float4*>(dst), make_float4(o[0], o[1], o[2], o[3]));
-            __stcs(reinterpret_cast<float4*>(dst) + 1, make_float4(o[4], o[5], o[6], o[7]));
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              if (2 * x0 + j < out_w) dst[j] = o[j];
-          }
-        }
-      }
-    }
-  }
-}
-
 // General path: any up/down/pad (incl. negative pads = crop) and any kernel size.
 __global__ void __launch_bounds__(256) upfirdn2d_general_kernel(const float* __restrict__ x, float* __restrict__ y,
                                                                 const float* __restrict__ k, int in_h, int in_w,
@@ -844,7 +379,6 @@ int launch_upfirdn2d(const float* x, float* y, const float* k, int planes, int i
   const int out_w = (in_w * up_x + px0 + px1 - kw) / down_x + 1;
   HF_REQUIRE(in_h * up_y + py0 + py1 - kh >= 0 && in_w * up_x + px0 + px1 - kw >= 0,
              "upfirdn2d: output would be empty (in %dx%d up %d pad %d,%d k %d)", in_h, in_w, up_y, py0, py1, kh);
-  if (planes == 0) return HF_OK;
   const bool k4 = (kh == 4 && kw == 4);
   const bool sym = (up_x == up_y && down_x == down_y);
   const bool pads03 = px0 >= 0 && py0 >= 0 && px1 >= 0 && py1 >= 0 && px0 <= 3 && px1 <= 3 && py0 <= 3 && py1 <= 3;
@@ -871,34 +405,6 @@ int launch_upfirdn2d(const float* x, float* y, const float* k, int planes, int i
              (reinterpret_cast<uintptr_t>(y) & 7) == 0) {
     if (in_w <= 512) bulk_go(upfirdn2d_up2_k4_bulk_kernel<2, 32, 6, 3>, 32, 6, 3);
     else bulk_go(upfirdn2d_up2_k4_bulk_kernel<4, 32, 6, 3>, 32, 6, 3);
-  } else if (k4 && sym && up_x == 1 && down_x == 1 && planes <= 65535 && px0 >= 0 && py0 >= 0 && px1 >= 0 && py1 >= 0) {
-    constexpr int RS = 64;                                   // rows per warp strip (3 halo rows each)
-    const int wx = out_w > 512 ? 8 : out_w > 256 ? 4 : out_w > 128 ? 2 : 1;   // warps side by side
-    dim3 grid(cdiv(out_w, 128 * wx), cdiv(out_h, RS * (8 / wx)), planes);
-    upfirdn2d_up1_k4_strip_kernel<RS><<<grid, 256, 0, st>>>(x, y, k, in_h, in_w, out_h, out_w, px0, py0, wx);
-  } else if (k4 && sym && up_x == 2 && down_x == 1 && planes <= 65535 && px0 == 2 && py0 == 2 && px1 == 1 &&
-             py1 == 1) {
-    constexpr int RS = 12;                                   // input rows per warp strip
-    const int wx = 1;              // warps stacked vertically (measured: 4.9 TB/s vs 4.5 side by side for 512-wide planes)
-    dim3 grid(cdiv(in_w, 128 * wx), cdiv(in_h, RS * (8 / wx)), planes);
-    upfirdn2d_up2_k4_strip_kernel<RS><<<grid, 256, 0, st>>>(x, y, k, in_h, in_w, wx);
-  } else if (k4 && sym && up_x == 1 && down_x == 2 && planes <= 65535 && px0 >= 0 && py0 >= 0 && px1 >= 0 && py1 >= 0) {
-    constexpr int RS = 16;                                   // 8 warps x 16 output rows x 128 output columns per CTA
-    dim3 grid(cdiv(out_w, 128), cdiv(out_h, 8 * RS), planes);
-    upfirdn2d_down2_k4_strip_kernel<RS><<<grid, 256, 0, st>>>(x, y, k, in_h, in_w, out_h, out_w, px0, py0);
-  } else if (k4 && sym && up_x == 1 && (down_x == 1 || down_x == 2) && planes <= 65535) {
-    if (down_x == 1) {
-      dim3 grid(cdiv(out_w, 64), cdiv(out_h, 32), planes);
-      upfirdn2d_up1_k4_kernel<1, 32><<<grid, 256, 0, st>>>(x, y, k, in_h, in_w, out_h, out_w, px0, py0);
-    } else {
-      dim3 grid(cdiv(out_w, 64), cdiv(out_h, 16), planes);
-      upfirdn2d_up1_k4_kernel<2, 16><<<grid, 256, 0, st>>>(x, y, k, in_h, in_w, out_h, out_w, px0, py0);
-    }
-  } else if (k4 && sym && up_x == 2 && down_x == 1 &&
-             (int64_t)planes * out_h * ((out_w + 3) / 4) < (int64_t)2000000000) {
-    int64_t quads = (int64_t)planes * out_h * ((out_w + 3) / 4);
-    int grid = (int)std::min<int64_t>((quads + 255) / 256, (int64_t)num_sms() * 32);
-    upfirdn2d_up2_k4_kernel<<<grid, 256, 0, st>>>(x, y, k, in_h, in_w, out_h, out_w, px0, py0, quads);
   } else {
     int64_t total = (int64_t)planes * out_h * out_w;
     int grid = (int)std::min<int64_t>((total + 255) / 256, (int64_t)num_sms() * 16);

@@ -28,84 +28,6 @@ __device__ __forceinline__ uint4 pack8s(const float* v) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Resnet18.conv1 (resnet.py:60,69): 7x7, stride 2, pad 3 on 3 channels.  K = 147 per output pixel is too thin for an
-// implicit-GEMM tap loop (Cin = 3 would be padded to 32 per tap: 11x wasted MMA work) and the first, direct SIMT
-// version ran at 30 TFLOP/s fp32 = 26 % of a BiSeNet forward.  So the stem is an explicit im2col into a 16-bit NHWC
-// tensor [B,Ho,Wo,160] (channel k = (c*7 + ky)*7 + kx, zero above 147 and outside the image) followed by the
-// ordinary 1x1 tensor-core convolution with the folded BatchNorm + ReLU epilogue.  One thread = 8 channels of one pixel.
-// ------------------------------------------------------------------------------------------------
-constexpr int kStemK = 147, kStemKPad = 160, kI2cTile = 128;
-
-template <int DT>
-__global__ void __launch_bounds__(256) im2col7x7s2_kernel(const float* __restrict__ x, uint16_t* __restrict__ y, int H,
-                                                          int W, int Ho, int Wo, int64_t total) {
-  // one CTA per output row (b, oy) (grid-stride): the only runtime-divisor divisions are per row; inside the row
-  // the (ox, 8-channel chunk) split divides by the constant 20
-  // The 21 input row segments (3 channels x 7 rows, zero filled outside the image) of a 128-pixel tile are staged in
-  // shared memory with coalesced loads; every thread then gathers 8 consecutive k from there.
-  __shared__ float sx[21][kI2cTile * 2 + 6];
-  const int plane = H * W;
-  const int rows = (int)total;                 // = B * Ho
-  constexpr int CH = kStemKPad / 8, SW = kI2cTile * 2 + 6;
-  const int xtiles = (Wo + kI2cTile - 1) / kI2cTile;
-  for (int work = blockIdx.x; work < rows * xtiles; work += gridDim.x) {
-    const int row = work / xtiles, ox0 = (work - row * xtiles) * kI2cTile;
-    const int b = row / Ho, oy = row - b * Ho;
-    const float* xb = x + (size_t)b * 3 * plane;
-    const int ybase = 2 * oy - 3, xbase = 2 * ox0 - 3;
-    __syncthreads();
-    // two unrolled phases: every global load of a thread is in flight before its first shared store
-    constexpr int N_STAGE = (21 * SW + 255) / 256;
-    float stage[N_STAGE];
-#pragma unroll
-    for (int it = 0; it < N_STAGE; ++it) {
-      const int i = threadIdx.x + it * 256;
-      const int rr = i / SW, q = i - rr * SW;
-      const int c = rr / 7, yy = ybase + (rr - c * 7), xx = xbase + q;
-      stage[it] = (i < 21 * SW && (unsigned)yy < (unsigned)H && (unsigned)xx < (unsigned)W)
-                      ? __ldg(xb + c * plane + yy * W + xx) : 0.f;
-    }
-#pragma unroll
-    for (int it = 0; it < N_STAGE; ++it) {
-      const int i = threadIdx.x + it * 256;
-      if (i < 21 * SW) sx[i / SW][i - (i / SW) * SW] = stage[it];
-    }
-    __syncthreads();
-    const int npix = min(kI2cTile, Wo - ox0);
-    uint16_t* ytile = y + ((size_t)row * Wo + ox0) * kStemKPad;
-    for (int idx = threadIdx.x; idx < npix * CH; idx += blockDim.x) {
-      const int oxl = idx / CH, k0 = (idx - oxl * CH) * 8;
-      int rr = k0 / 7, kx = k0 - rr * 7;             // rr = c*7 + ky; walk kx fastest
-      float v[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        v[j] = rr < 21 ? sx[rr][2 * oxl + kx] : 0.f;
-        if (++kx == 7) { kx = 0; ++rr; }
-      }
-      *reinterpret_cast<uint4*>(ytile + (size_t)idx * 8) = pack8s<DT>(v);
-    }
-  }
-}
-
-int launch_im2col7x7s2(const float* x, void* y16, int B, int H, int W, int dtype, cudaStream_t st) {
-  HF_REQUIRE(x && y16, "im2col7x7s2: null pointer");
-  HF_REQUIRE(B > 0 && H > 0 && W > 0, "im2col7x7s2: bad shape");
-  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-  const int64_t total = (int64_t)B * Ho;         // output rows
-  HF_REQUIRE(total < (int64_t)2000000000, "tensor too large for one launch (%lld rows): split the batch", (long long)total);
-  const int64_t work = total * ((Wo + kI2cTile - 1) / kI2cTile);
-  HF_REQUIRE(work < (int64_t)2000000000, "im2col7x7s2: too many tiles (%lld): split the batch", (long long)work);
-  const int grid = (int)std::min<int64_t>(work, (int64_t)num_sms() * 16);
-  if (dtype == HF_BF16)
-    im2col7x7s2_kernel<HF_BF16><<<grid, 256, 0, st>>>(x, (uint16_t*)y16, H, W, Ho, Wo, total);
-  else
-    im2col7x7s2_kernel<HF_F16><<<grid, 256, 0, st>>>(x, (uint16_t*)y16, H, W, Ho, Wo, total);
-  HF_LAUNCH_OK("im2col7x7s2");
-  count_launch();
-  return HF_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
 // nn.MaxPool2d(kernel_size=3, stride=2, padding=1) (resnet.py:62,71) on NHWC 16-bit; padding never wins the max.
 // ------------------------------------------------------------------------------------------------
 template <int DT>
@@ -256,13 +178,13 @@ int launch_gate_add_up(const void* x16, const float* gate, const float* addvec, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Fused stem (round 2): Resnet18.conv1 7x7/s2/p3 + bn1 + ReLU (resnet.py:60-61,69-70) in ONE kernel, fp32 NCHW image in,
-// 16-bit NHWC [B,Ho,Wo,64] out -- the [B,Ho,Wo,160] im2col tensor (21 MB per 512^2 image, written by one kernel and
-// read back by the next: 0.84 ms of a B=48 call) no longer exists.
+// Fused stem: Resnet18.conv1 7x7/s2/p3 + bn1 + ReLU (resnet.py:60-61,69-70) in ONE kernel, fp32 NCHW image in,
+// 16-bit NHWC [B,Ho,Wo,64] out.  It is not an hf_conv2d_forward layer: with 3 input channels the implicit-GEMM tap loop
+// would pad each tap's K to 32 (11x wasted MMA work), and no intermediate patch tensor is written to HBM.
 // Roofline: 1.23 GFLOP against 3 MB in + 8.4 MB out per 512^2 image = 108 FLOP/B, far left of the ridge (~260): the
 // kernel is HBM-bound, so the contraction runs on warp-level mma.sync.m16n8k16 fragments built straight from a
 // shared-memory copy of the input window (K = 7 rows x 24 [= 7 taps x 3 channels + 3 zero-weight pads] = 168 -> 176);
-// a tensor-core tile would need the same im2col rows materialised in the swizzled operand layout first.
+// a wgmma tile would need the same patch rows materialised in the swizzled operand layout first.
 // CTA = 8 x 32 output pixels x 64 channels, 8 warps (one output row each: 2 m16 tiles x 8 n8 tiles x 11 k16 steps).
 // ------------------------------------------------------------------------------------------------
 constexpr int kSfRows = 8, kSfCols = 32;                 // output tile

@@ -273,11 +273,6 @@ int hf_stem3x3_nhwc16(const float* x, const void* wpacked, const float* shift, c
 int hf_stem7x7s2_nhwc16(const float* x, const void* wpacked, const float* shift, void* y16, int batch, int height,
                         int width, int dtype, void* stream);
 
-/* im2col for Resnet18.conv1 (resnet.py:60,69; 7x7 / stride 2 / pad 3 on 3 channels): x [B,3,H,W] fp32 NCHW ->
- * y16 [B,Ho,Wo,160] 16-bit NHWC, channel k = (c*7 + ky)*7 + kx (= the flattening of the conv weight [64,3,7,7]),
- * zero for k >= 147 and outside the image; Ho = (H-1)/2+1.  The stem is then hf_conv2d_forward with
- * {cin 147, cin_pad 160, ksize 1} and the folded bn1 + ReLU epilogue. */
-int hf_im2col7x7s2_nhwc16(const float* x, void* y16, int batch, int height, int width, int dtype, void* stream);
 /* nn.MaxPool2d(3, 2, 1) (resnet.py:62,71) on 16-bit NHWC; output (H-1)/2+1 x (W-1)/2+1 */
 int hf_maxpool3x3s2_nhwc16(const void* x16, void* y16, int batch, int height, int width, int channels, int dtype,
                            void* stream);

@@ -83,7 +83,7 @@ def test_upfirdn2d_bulk_paths_vs_oracle(op, shape, up, down, pad, separable):
     y = op.upfirdn2d(x.cuda(), k.cuda(), up=up, down=down, pad=pad)
     assert y.shape == ref.shape
     assert float((y.cpu() - ref).abs().max()) < TOL_FP32 * 4
-    # the same call on a 4-byte-offset view takes the ring / register-window kernels instead: both paths must agree
+    # the same call on a 4-byte-offset view takes the general kernel instead: both paths must agree
     buf = torch.empty(x.numel() + 1, device="cuda")
     xv = buf[1:].view(shape)
     xv.copy_(x)
@@ -93,7 +93,7 @@ def test_upfirdn2d_bulk_paths_vs_oracle(op, shape, up, down, pad, separable):
 
 def test_upfirdn2d_blur_full_size_both_paths(op):
     """The north_star blur shape [B*C, 1025, 1025] -> 1024^2 (model.py:252-263) at full size: TMA bulk path vs the
-    ring kernel on an unaligned view of the same data, plus the DC gain of the normalised FIR in the interior."""
+    general kernel on an unaligned view of the same data, plus the DC gain of the normalised FIR in the interior."""
     k = (O.make_kernel([1, 3, 3, 1]) * 4).cuda()
     x = torch.randn(1, 8, 1025, 1025, device="cuda")
     y = op.upfirdn2d(x, k / 4, up=1, down=1, pad=(1, 1))
