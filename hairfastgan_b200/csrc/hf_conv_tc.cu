@@ -13,10 +13,13 @@
 // channel chunks.  One TMA box per (tap, channel chunk), shifted by the tap offset, brings the activations into a
 // swizzled K-major ring slot next to the matching weight box; TMA out-of-bounds zero fill *is* the conv zero
 // padding, and the 128 GEMM rows may span several batch samples (4x4x8, 8x8x2).  Stride 2 walks every other input
-// pixel through TMA element strides.
+// pixel through TMA element strides.  Stride-1 3x3 convolutions on 16 x 8 tiles of one sample instead load one
+// (8 + 2) x 16 box per (channel chunk, column shift) into a separate activation ring and take its three row shifts
+// from row offsets 0 / 16 / 32 of it (ConvPlan::shift_boxes): 3 x 10/8 instead of 9 activation boxes per chunk.
 //
 // conv_wgmma_kernel: persistent CTAs with a static schedule, three warpgroups.  Warpgroup 0 is the TMA producer
-// (one thread); warpgroups 1 and 2 each own 64 of the 128 GEMM rows, issue wgmma m64 x n_tile x k16 with the
+// (one thread, registers handed to the consumers with setmaxnreg); warpgroups 1 and 2 each own 64 of the 128 GEMM
+// rows, issue wgmma m64 x n_tile x k16 with the
 // fp32 accumulator in registers, release ring slots through mbarriers as their MMAs retire, and run the fused
 // epilogue: the accumulator goes through a padded fp32 staging tile in shared memory so that one thread sees
 // 32 consecutive channels of one pixel (two threads per pixel, alternating 32-channel chunks).  While the
@@ -33,6 +36,7 @@
 namespace hf {
 
 constexpr int kMaxStages = 8;
+constexpr int kShiftASlots = 2;      // activation ring depth of the column-shift path (each slot feeds 3 k-blocks)
 constexpr int kMaxDynSmem = 232448;   // 227 KB: opt-in dynamic shared memory per block on sm_90
 constexpr int kTableBytes = 16384;   // 512 entries x 32 B
 constexpr float kSqrt2 = 1.41421356237309515f;
@@ -46,8 +50,10 @@ struct ConvKernelParams {
   int num_m_tiles;
   int num_kb;              // taps * Cin / KCHUNK
   int kc_per_tap;          // Cin / KCHUNK
-  int stages;              // A+B ring stages
+  int stages;              // A+B ring stages (B only with shift_boxes)
   uint32_t stage_bytes, a_bytes;
+  int shift_boxes;         // ConvPlan::shift_boxes: the activation ring precedes the B ring
+  uint32_t a_slot_bytes;   // one (TH + 2) x TW x KCHUNK activation box
   const float* d;
   const float* noise;
   int64_t noise_bstride;
@@ -358,10 +364,13 @@ constexpr int kConvThreads = 384;     // warpgroup 0: TMA producer; warpgroups 1
 constexpr int kStagePad = 4;          // staging row pitch = n_tile + 4 floats
 constexpr int kMaxNTile = 128;        // m64 x n128 fp32 accumulator = 64 registers per thread
 
-// shared memory besides the ring: staging tiles, two epilogue tables, ToRGB exchange, barriers
+constexpr int kProducerRegs = 40;      // setmaxnreg: 128 x 40 + 256 x 232 = 384 x 168 (the __launch_bounds__ cap)
+constexpr int kConsumerRegs = 232;
+
+// shared memory besides the rings: staging tiles, two epilogue tables, ToRGB exchange, barriers
 __host__ __device__ constexpr size_t conv_fixed_smem(int n_tile) {
   return 1024 /*align*/ + (size_t)2 * 64 * (n_tile + kStagePad) * 4 + 2 * (size_t)kTableBytes + 2 * 64 * 4 * 4 +
-         2 * kMaxStages * 8;
+         2 * (kMaxStages + kShiftASlots) * 8;
 }
 
 template <int KCHUNK, int DT, int NT>
@@ -371,12 +380,16 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int SP = NT + kStagePad;
-  uint8_t* stage_base = smem;
-  float* staging = reinterpret_cast<float*>(smem + (size_t)p.stages * p.stage_bytes);           // [2][64][SP]
+  const uint32_t ring_a_bytes = p.shift_boxes ? kShiftASlots * p.a_slot_bytes : 0u;
+  uint8_t* a_ring = smem;                                                    // [kShiftASlots] (shift_boxes only)
+  uint8_t* stage_base = smem + ring_a_bytes;
+  float* staging = reinterpret_cast<float*>(stage_base + (size_t)p.stages * p.stage_bytes);      // [2][64][SP]
   TableEntry* tables = reinterpret_cast<TableEntry*>(staging + 2 * 64 * SP);                     // [2][512]
   float* rgbx = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(tables) + 2 * kTableBytes);  // [2][64][4]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(rgbx + 2 * 64 * 4);                           // [kMaxStages]
   uint64_t* empty_bar = full_bar + kMaxStages;                                                   // [kMaxStages]
+  uint64_t* a_full_bar = empty_bar + kMaxStages;                                                 // [kShiftASlots]
+  uint64_t* a_empty_bar = a_full_bar + kShiftASlots;                                             // [kShiftASlots]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -391,32 +404,61 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8);                 // lane 0 of each of the eight consumer warps
     }
+    for (int s = 0; s < kShiftASlots; ++s) {
+      mbar_init(&a_full_bar[s], 1);
+      mbar_init(&a_empty_bar[s], 8);
+    }
     mbar_fence_init();
   }
   __syncthreads();
 
   if (warp < 4) {
     // ================================ TMA producer ================================
+    setmaxnreg_dec<kProducerRegs>();
     if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
+      int a_stage = 0;
+      uint32_t a_phase = 0;
       const int pad = (p.taps == 9) ? 1 : 0;
-      const uint32_t tx_bytes = p.stage_bytes;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         const int nt = tile % p.num_n_tiles;
         const MTile tc = decode_mtile(p, tile / p.num_n_tiles);
         const int b0 = tc.bt * p.TB, n0 = nt * p.n_tile;
         const int c_off = (n0 / p.cout_g) * p.cin_g;        // grouped weights: this N tile's input channels
+        if (p.shift_boxes) {
+          // k order (chunk, dx, dy): one (TH + 2)-row box per (chunk, dx), then the weight boxes of its three taps
+          for (int kc = 0; kc < p.kc_per_tap; ++kc) {
+            for (int dx = 0; dx < 3; ++dx) {
+              mbar_wait_nocall(&a_empty_bar[a_stage], a_phase ^ 1);
+              mbar_expect_tx(&a_full_bar[a_stage], p.a_slot_bytes);
+              tma_load_4d(a_ring + (size_t)a_stage * p.a_slot_bytes, &tmA, &a_full_bar[a_stage],
+                          c_off + kc * KCHUNK, tc.x0 + dx - 1, tc.y0 - 1, b0);
+              if (++a_stage == kShiftASlots) { a_stage = 0; a_phase ^= 1; }
+              for (int dy = 0; dy < 3; ++dy) {
+                mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
+                mbar_expect_tx(&full_bar[stage], p.stage_bytes);
+                tma_load_2d(stage_base + (size_t)stage * p.stage_bytes, &tmB, &full_bar[stage],
+                            (dy * 3 + dx) * p.cin_g + kc * KCHUNK, n0);
+                if (++stage == p.stages) { stage = 0; phase ^= 1; }
+              }
+            }
+          }
+          continue;
+        }
         for (int tap = 0; tap < p.taps; ++tap) {
           const int dy = (p.taps == 9) ? tap / 3 : 0, dx = (p.taps == 9) ? tap % 3 : 0;
           for (int kc = 0; kc < p.kc_per_tap; ++kc) {
             mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
             uint8_t* a_dst = stage_base + (size_t)stage * p.stage_bytes;
             uint8_t* b_dst = a_dst + p.a_bytes;
-            mbar_expect_tx(&full_bar[stage], tx_bytes);
+            // debug probe (p.dbg & 2): activations for the centre tap only -> WRONG outputs, 1/9 of the A traffic
+            const bool load_a = !(p.dbg & 2) || tap == p.taps / 2;
+            mbar_expect_tx(&full_bar[stage], load_a ? p.stage_bytes : p.stage_bytes - p.a_bytes);
             // stride 2: the tensor map walks every other input pixel (TMA element strides)
-            tma_load_4d(a_dst, &tmA, &full_bar[stage], c_off + kc * KCHUNK, tc.x0 * p.stride + dx - pad,
-                        tc.y0 * p.stride + dy - pad, b0);
+            if (load_a)
+              tma_load_4d(a_dst, &tmA, &full_bar[stage], c_off + kc * KCHUNK, tc.x0 * p.stride + dx - pad,
+                          tc.y0 * p.stride + dy - pad, b0);
             tma_load_2d(b_dst, &tmB, &full_bar[stage], tap * p.cin_g + kc * KCHUNK, n0);
             if (++stage == p.stages) { stage = 0; phase ^= 1; }
           }
@@ -427,6 +469,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   }
 
   // ================================ consumers: MMA + epilogue ============================
+  setmaxnreg_inc<kConsumerRegs>();
   const int cg = (threadIdx.x >> 7) - 1;       // GEMM rows [64 cg, 64 cg + 64)
   const int t = threadIdx.x & 127;
   const int cw = t >> 5;                       // warp within the warpgroup: accumulator rows [16 cw, 16 cw + 16)
@@ -443,8 +486,11 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const size_t plane_o = (size_t)p.Ho * p.Wo;
   const uint32_t a_off = (uint32_t)cg * 64u * ROW_BYTES;
   const uint32_t smem_base_u32 = smem_u32(stage_base);
+  const uint32_t a_ring_u32 = smem_u32(a_ring);
   int stage = 0;
   uint32_t phase = 0;
+  int a_stage = 0;
+  uint32_t a_phase = 0;
   int cached_bt = -1, cached_nt = -1;
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
     const int nt = tile % p.num_n_tiles;
@@ -463,12 +509,19 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     float acc[NT / 2];
 #pragma unroll
     for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
-    int prev = -1;
+    int prev = -1, prev_a = -1;
+    int dy = 0;                                     // shift_boxes: row shift of this k-block (k order chunk, dx, dy)
     for (int kb = 0; kb < p.num_kb; ++kb) {
+      const uint32_t s_addr = smem_base_u32 + (uint32_t)stage * p.stage_bytes;
+      uint32_t a_addr = s_addr;
+      if (p.shift_boxes) {
+        if (dy == 0) mbar_wait_nocall(&a_full_bar[a_stage], a_phase);
+        // row shift dy = the box rows [16 dy, 16 dy + 128): whole swizzle atoms, so only the start address moves
+        a_addr = a_ring_u32 + (uint32_t)a_stage * p.a_slot_bytes + (uint32_t)(dy * 16) * ROW_BYTES;
+      }
       mbar_wait_nocall(&full_bar[stage], phase);
-      const uint32_t a_addr = smem_base_u32 + (uint32_t)stage * p.stage_bytes;
       const uint64_t da = make_gmma_desc(a_addr + a_off, SBO, LAYOUT);
-      const uint64_t db = make_gmma_desc(a_addr + p.a_bytes, SBO, LAYOUT);
+      const uint64_t db = make_gmma_desc(s_addr + p.a_bytes, SBO, LAYOUT);
       wgmma_fence_regs(acc);
       wgmma_fence();
 #pragma unroll
@@ -479,10 +532,20 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       prev = stage;
       if (++stage == p.stages) { stage = 0; phase ^= 1; }
+      if (p.shift_boxes) {
+        // the previous box's last (dy = 2) k-block has retired too
+        if (dy == 0 && prev_a >= 0 && lane == 0) mbar_arrive(&a_empty_bar[prev_a]);
+        if (++dy == 3) {
+          dy = 0;
+          prev_a = a_stage;
+          if (++a_stage == kShiftASlots) { a_stage = 0; a_phase ^= 1; }
+        }
+      }
     }
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
     if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    if (prev_a >= 0 && lane == 0) mbar_arrive(&a_empty_bar[prev_a]);
 
     // accumulator fragment -> staging rows (m64nNk16: row 16*warp + lane/4 (+8), columns 8j + 2*(lane%4) (+1))
     {
@@ -509,7 +572,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // ---------------------------------------------------------------------------------------------
 int conv_up_nc(int Cout) { return Cout < 32 ? Cout : 32; }
 
-// Experiment knobs (HF_CONV_DBG: drop the epilogue -> WRONG outputs) exist only in
+// Experiment knobs (HF_CONV_DBG bit 0: drop the epilogue; bit 1: per-tap mainloop only, load the activation box of
+// the centre tap only, to see whether the L2 -> shared-memory feed limits it -- both give WRONG outputs) exist only in
 // -DHF_DEBUG builds; the shipped library never reads the environment on the launch path.
 #ifdef HF_DEBUG
 static int env_int(const char* name, int dflt) {
@@ -568,15 +632,21 @@ int conv_plan(const ConvLaunch& a, ConvPlan* p) {
   p->n_tile = n_tile;
   p->num_n_tiles = ntot / n_tile;
   p->nc = a.up ? n_tile / 4 : n_tile;
+  // Stride-1 3x3 convolutions over one 16-pixel-wide, 8-row tile of one sample: the three row shifts of a column
+  // shift read the same (8 + 2) x 16 pixel box, so one box per (chunk, dx) replaces three per-tap boxes and the
+  // activation traffic from L2 drops from 9 to 3 x 10/8 boxes per chunk.
+  p->shift_boxes = a.taps == 9 && stride == 1 && p->TW == 16 && p->TB == 1;
   const size_t fixed = conv_fixed_smem(n_tile);
-  const size_t budget = kMaxDynSmem - fixed;
   const int row_bytes = p->kchunk * 2;
-  const size_t stage_bytes = (size_t)128 * row_bytes + (size_t)n_tile * row_bytes;
+  p->a_slot_bytes = p->shift_boxes ? (uint32_t)((p->TH + 2) * p->TW * row_bytes) : 0u;
+  const size_t ring_a = (size_t)kShiftASlots * p->a_slot_bytes;
+  const size_t budget = kMaxDynSmem - fixed - ring_a;
+  const size_t stage_bytes = (p->shift_boxes ? 0 : (size_t)128 * row_bytes) + (size_t)n_tile * row_bytes;
   int stages = (int)(budget / stage_bytes);
   if (stages > kMaxStages) stages = kMaxStages;
   HF_REQUIRE(stages >= 2, "conv: not enough shared memory for 2 stages");
   p->stages = stages;
-  p->smem_bytes = fixed + stages * stage_bytes;
+  p->smem_bytes = fixed + ring_a + stages * stage_bytes;
   p->num_tiles = p->num_m_tiles * p->num_n_tiles;
   p->grid = p->num_tiles < sms ? p->num_tiles : sms;
   return HF_OK;
@@ -617,6 +687,7 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
     uint32_t es[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
     // stride 2: the box is traversed with element stride 2, so it must span 2*T elements to deliver T samples
     if (stride == 2) { box[1] = (uint32_t)pl.TW * 2; box[2] = (uint32_t)pl.TH * 2; }
+    if (pl.shift_boxes) box[2] = (uint32_t)pl.TH + 2;        // the rows above and below the tile (row shifts)
     rc = encode_tmap(&tmA, a.dtype, 4, const_cast<void*>(a.xhat_in), dims, strides, box, pl.kchunk * 2,
                      stride == 2 ? es : nullptr);
     if (rc) return rc;
@@ -643,8 +714,10 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
   kp.kc_per_tap = cin_g / pl.kchunk;
   kp.num_kb = a.taps * kp.kc_per_tap;
   kp.stages = pl.stages;
-  kp.a_bytes = 128u * pl.kchunk * 2;
+  kp.a_bytes = pl.shift_boxes ? 0u : 128u * pl.kchunk * 2;
   kp.stage_bytes = kp.a_bytes + (uint32_t)pl.n_tile * pl.kchunk * 2;
+  kp.shift_boxes = pl.shift_boxes;
+  kp.a_slot_bytes = pl.a_slot_bytes;
   kp.d = a.d;
   kp.noise = a.noise;
   kp.noise_bstride = (a.noise && a.noise_batch > 1) ? (int64_t)kp.Ho * kp.Wo : 0;
@@ -656,7 +729,7 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
   kp.rgb_w = a.rgb_partial ? a.rgb_w : nullptr;
   kp.rgb_s = a.rgb_s;
   kp.rgb_partial = a.rgb_partial;
-  kp.dbg = env_int("HF_CONV_DBG", 0);       // experiments only: 1 = epilogue reduced to the accumulator read
+  kp.dbg = env_int("HF_CONV_DBG", 0);       // experiments only, see env_int
   kp.epi = a.epi; kp.stride = stride; kp.cin_g = cin_g; kp.enc_post = a.enc_post;
   kp.cout_g = (a.up ? 4 * a.Cout : a.Cout) / groups;
   kp.enc_act = a.enc_act; kp.enc_slope0 = a.enc_slope0;

@@ -131,19 +131,23 @@ struct ConvLaunch {
   void* enc_y16b;
 };
 struct ConvPlan {
-  // halo, G, na_slots, pitch, b_resident, a_slot_bytes: halo-tile scheduling fields of the plan query ABI
-  // (hf_conv_plan_query); conv_wgmma_kernel loads one box per (tap, channel chunk) and reports 0 / 1 / 0 / 0 / 0 / 0.
+  // halo, G, na_slots, pitch, b_resident: fields of the plan query ABI (hf_conv_plan_query) that described the
+  // resident-halo scheduler of the B200 kernel this one replaced; conv_wgmma_kernel has no such scheduler and always
+  // reports 0 / 1 / 0 / 0 / 0.  The column-shift boxes below are a different scheme and do not use them.
   int halo;
   int G;
   int ng;                 // consumer warpgroups (MMA + epilogue), 64 GEMM rows each
   int na_slots, pitch;
   int b_resident;
+  // 1: one (TH + 2)-row activation box per (channel chunk, column shift) serves the three row shifts; activation
+  // boxes and weight boxes then have separate rings (kShiftASlots slots of a_slot_bytes; `stages` weight slots)
+  int shift_boxes;
   uint32_t a_slot_bytes;
   int TW, TH, TB;         // pixel tile: TW*TH*TB = 128 GEMM rows
   int tiles_x, tiles_y, tiles_b, num_m_tiles;
   int n_tile, num_n_tiles, nc;
   int kchunk;             // channels per pipeline stage (64 -> SWIZZLE_128B, 32 -> SWIZZLE_64B)
-  int stages;
+  int stages;             // ring slots: (activation + weight) boxes, or weight boxes only with shift_boxes
   size_t smem_bytes;
   int num_tiles, grid;
 };
