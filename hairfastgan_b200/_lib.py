@@ -45,6 +45,10 @@ class hf_conv2d_io(C.Structure):
                 ("act_after_residual", C.c_int)]
 
 
+class hf_sean_ace_tables(C.Structure):
+    _fields_ = [("fc_w", C.c_void_p), ("fc_b", C.c_void_p), ("tw", C.c_void_p), ("table", C.c_void_p), ("n2", C.c_int)]
+
+
 class hf_gen_config(C.Structure):
     _fields_ = [("size", C.c_int), ("style_dim", C.c_int), ("channel_multiplier", C.c_int), ("dtype", C.c_int)]
 
@@ -133,7 +137,15 @@ SYMBOLS = {
     "hf_fspace_blend_f32": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_float),
                                       C.POINTER(C.c_float), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                       C.c_int, C.c_void_p]),
-    "hf_generator_packed_bytes": (C.c_size_t, [C.POINTER(hf_gen_config)]),
+    "hf_sean_labels": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "hf_sean_onehot_conv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                      C.c_int, C.c_void_p]),
+    "hf_sean_style_tables": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(hf_sean_ace_tables), C.c_int, C.c_void_p,
+                                       C.c_void_p]),
+    "hf_sean_ace_apply": (C.c_int, [C.c_void_p] * 8 + [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "hf_sean_conv_img": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                   C.c_void_p]),
+    "hf_generator_packed_bytes":(C.c_size_t, [C.POINTER(hf_gen_config)]),
     "hf_generator_workspace_bytes": (C.c_size_t, [C.POINTER(hf_gen_config), C.c_int]),
     "hf_generator_pack": (C.c_int, [C.POINTER(hf_gen_config), C.POINTER(hf_gen_weights), C.c_void_p, C.c_void_p]),
     "hf_generator_forward": (C.c_int, [C.POINTER(hf_gen_config), C.c_void_p, C.POINTER(hf_gen_io), C.c_void_p,

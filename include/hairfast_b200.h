@@ -328,6 +328,51 @@ int hf_fspace_blend_f32(const float* first, const float* const* src, const float
                         const float* scale_b, float* out, int n_stage, int channels, int height, int width,
                         int mask_height, int mask_width, void* stream);
 
+/* ---- SEAN decode_sean (models/sean_codes/models/pix2pix_model.py:309-325, UI_mode, batch 1) ----
+ * The SPADE generator's block convolutions run on hf_conv2d_forward; these calls supply the rest. */
+
+/* labels: int64 [size,size] (the `target_mask` label values) -> maps: int8 label maps at R = size/32, size/16, ..., size
+ * concatenated in that order (R = 8..256 for size 256), L_R[y,x] = label[y*size/R, x*size/R] (F.interpolate nearest,
+ * generator.py:75, normalization.py:115).  *bad (device int) = number of labels outside 0..18. */
+int hf_sean_labels(const long long* labels, int8_t* maps, int* bad, int size, void* stream);
+
+/* 3x3 zero-padded convolution of the one-hot map of `labels` [res,res] (19 classes) as a table lookup:
+ * y16[p,c] = act(bias[c] + sum_{tap, p+tap inside} table[tap][L(p+tap)][c]); table [9][19][channels] fp32 =
+ * weight[c, j, ky, kx] at tap = ky*3 + kx; bias [channels] or NULL; act 0 none / 3 ReLU; y16 [res,res,channels]
+ * 16-bit NHWC.  SPADEGenerator.fc (generator.py:33,75-76) and every SPADE.mlp_shared (normalization.py:241-253). */
+int hf_sean_onehot_conv(const int8_t* labels, const float* table, const float* bias, int act, void* y16, int res,
+                        int channels, int dtype, void* stream);
+
+/* One ACE layer's style-table operands (all fp32, device). */
+typedef struct {
+  const float* fc_w;   /* [19][512][512]: fc_mu{j}.weight */
+  const float* fc_b;   /* [19][512]: fc_mu{j}.bias */
+  const float* tw;     /* [9*n2][512]: row tap*n2 + n = [a_g conv_gamma.weight; a_b conv_beta.weight][n, :, tap] */
+  float* table;        /* out: [19][9][n2] */
+  int n2;              /* 2 * norm_nc */
+} hf_sean_ace_tables;
+
+/* Per-call style tables of n_ace (<= 16) ACE layers in two launches:
+ * code_j = image_code[j] ([19][512]) unless that row is all zero, then mean_code[j] (pix2pix_model.py:312-315);
+ * mu_j = relu(fc_w[j] . code_j + fc_b[j]) (normalization.py:133-135); table[j][tap][n] = tw[tap*n2 + n] . mu_j.
+ * aces: HOST array; mu_workspace: n_ace * 19 * 512 floats. */
+int hf_sean_style_tables(const float* image_code, const float* mean_code, const hf_sean_ace_tables* aces, int n_ace,
+                         float* mu_workspace, void* stream);
+
+/* ACE.forward (normalization.py:108-189) + optional leaky_relu(0.2) (architecture.py:95-96), batch 1:
+ * v = (x + noise[w*res + h] * noise_var[c]) * bn_scale[c] + bn_shift[c]; g / b = gamma_beta[c] / gamma_beta[C + c]
+ * (+ sum over valid taps of table[L(p+tap)][tap][c] / [C + c] when table != NULL); out = v * (1 + g) + b.
+ * x16 / y16 [res,res,channels] 16-bit NHWC; noise [res*res] (torch.randn(1, W, H, 1)); gamma_beta [2C,res,res] fp32
+ * NCHW; table [19][9][2C] fp32 (hf_sean_style_tables) or NULL; labels [res,res].  res^2 % 32 == 0, channels % 64 == 0. */
+int hf_sean_ace_apply(const void* x16, const float* noise, const float* noise_var, const float* bn_scale,
+                      const float* bn_shift, const float* gamma_beta, const float* table, const int8_t* labels,
+                      int lrelu, void* y16, int res, int channels, int dtype, void* stream);
+
+/* tanh(conv_img(leaky_relu(x, 0.2))) (generator.py:107-108): x16 [res,res,channels] 16-bit NHWC, weight [3][channels]
+ * [3][3], bias [3] -> y [3,res,res] fp32 NCHW.  channels % 8 == 0, <= 256. */
+int hf_sean_conv_img(const void* x16, const float* weight, const float* bias, float* y, int res, int channels,
+                     int dtype, void* stream);
+
 /* Number of kernels the last hf_generator_forward / hf_conv_forward of this thread launched. */
 int hf_last_launch_count(void);
 /* Number of kernels every hf_* call of this thread has launched since the library was loaded. */
