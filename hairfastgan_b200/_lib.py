@@ -102,6 +102,7 @@ SYMBOLS = {
     "hf_conv2d_packed_bytes": (C.c_size_t, [C.POINTER(hf_conv2d_desc)]),
     "hf_conv2d_pack": (C.c_int, [C.POINTER(hf_conv2d_desc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "hf_conv2d_forward": (C.c_int, [C.POINTER(hf_conv2d_desc), C.c_void_p, C.POINTER(hf_conv2d_io), C.c_void_p]),
+    "hf_conv2d_plan_query": (C.c_int, [C.POINTER(hf_conv2d_desc), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]),
     "hf_nchw_to_nhwc16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_int, C.c_void_p]),
     "hf_nhwc16_to_nchw": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),

@@ -193,9 +193,7 @@ int hf_conv_plan_query(const hf_conv_desc* d, int batch, int height, int width, 
   cl.taps = d->ksize * d->ksize; cl.up = d->upsample; cl.dtype = d->dtype;
   ConvPlan pl;
   if ((rc = conv_plan(cl, &pl))) return rc;
-  const int v[12] = {pl.halo, pl.n_tile, pl.num_n_tiles, pl.G, pl.na_slots, pl.pitch, pl.b_resident, pl.stages,
-                     (int)pl.smem_bytes, pl.num_tiles, pl.grid, pl.kchunk};
-  for (int i = 0; i < 12; ++i) out[i] = v[i];
+  conv_plan_export(pl, out);
   return HF_OK;
 }
 

@@ -617,14 +617,10 @@ int conv_plan(const ConvLaunch& a, ConvPlan* p) {
   const int table_cap = kTableBytes / (int)sizeof(TableEntry);   // entries per consumer warpgroup
   const int tb_rows = a.epi == 1 ? 1 : p->TB;      // encoder epilogue tables are per channel only
   int n_tile = 0;
-  if (a.force_n_tile) {
-    n_tile = a.force_n_tile;
-  } else {
-    for (int cand = kMaxNTile; cand >= nmin; cand >>= 1) {
-      if (cout_g % cand || tb_rows * (a.up ? cand / 4 : cand) > table_cap) continue;
-      n_tile = cand;
-      if ((int64_t)p->num_m_tiles * (ntot / cand) >= sms) break;   // largest tile that still fills the GPU
-    }
+  for (int cand = kMaxNTile; cand >= nmin; cand >>= 1) {
+    if (cout_g % cand || tb_rows * (a.up ? cand / 4 : cand) > table_cap) continue;
+    n_tile = cand;
+    if ((int64_t)p->num_m_tiles * (ntot / cand) >= sms) break;   // largest tile that still fills the GPU
   }
   HF_REQUIRE(n_tile >= nmin && n_tile <= kMaxNTile && cout_g % n_tile == 0 && n_tile % 32 == 0 &&
                  tb_rows * (a.up ? n_tile / 4 : n_tile) <= table_cap,
@@ -639,6 +635,7 @@ int conv_plan(const ConvLaunch& a, ConvPlan* p) {
   const size_t fixed = conv_fixed_smem(n_tile);
   const int row_bytes = p->kchunk * 2;
   p->a_slot_bytes = p->shift_boxes ? (uint32_t)((p->TH + 2) * p->TW * row_bytes) : 0u;
+  p->na_slots = p->shift_boxes ? kShiftASlots : 0;
   const size_t ring_a = (size_t)kShiftASlots * p->a_slot_bytes;
   const size_t budget = kMaxDynSmem - fixed - ring_a;
   const size_t stage_bytes = (p->shift_boxes ? 0 : (size_t)128 * row_bytes) + (size_t)n_tile * row_bytes;
@@ -650,6 +647,12 @@ int conv_plan(const ConvLaunch& a, ConvPlan* p) {
   p->num_tiles = p->num_m_tiles * p->num_n_tiles;
   p->grid = p->num_tiles < sms ? p->num_tiles : sms;
   return HF_OK;
+}
+
+void conv_plan_export(const ConvPlan& pl, int* out) {
+  const int v[12] = {pl.halo, pl.n_tile, pl.num_n_tiles, pl.G, pl.na_slots, pl.pitch, pl.b_resident, pl.stages,
+                     (int)pl.smem_bytes, pl.num_tiles, pl.grid, pl.kchunk};
+  for (int i = 0; i < 12; ++i) out[i] = v[i];
 }
 
 template <int KCHUNK, int DT>

@@ -21,6 +21,18 @@ static int check_conv2d(const hf_conv2d_desc* d) {
   return HF_OK;
 }
 
+// the shape half of the launch: what conv_plan reads
+static ConvLaunch conv2d_launch_shape(const hf_conv2d_desc* d, int batch, int height, int width) {
+  ConvLaunch cl;
+  memset(&cl, 0, sizeof(cl));
+  cl.B = batch; cl.H = height; cl.W = width;
+  cl.Cin = d->cin_pad; cl.Cout = d->cout;
+  cl.taps = d->ksize * d->ksize; cl.dtype = d->dtype;
+  cl.stride = d->stride; cl.groups = d->groups;
+  cl.epi = 1;
+  return cl;
+}
+
 extern "C" {
 
 size_t hf_conv2d_packed_bytes(const hf_conv2d_desc* d) {
@@ -46,14 +58,8 @@ int hf_conv2d_forward(const hf_conv2d_desc* d, const void* packed, const hf_conv
   HF_REQUIRE(io->y16 || io->y16b || io->y32_nchw, "hf_conv2d_forward: no output requested");
   HF_REQUIRE(io->batch > 0 && io->height > 0 && io->width > 0, "hf_conv2d_forward: bad shape");
   HF_REQUIRE(io->act != 1 || io->slope, "hf_conv2d_forward: PReLU needs a slope vector");
-  ConvLaunch cl;
-  memset(&cl, 0, sizeof(cl));
-  cl.B = io->batch; cl.H = io->height; cl.W = io->width;
-  cl.Cin = d->cin_pad; cl.Cout = d->cout;
-  cl.taps = d->ksize * d->ksize; cl.dtype = d->dtype;
-  cl.stride = d->stride; cl.groups = d->groups;
+  ConvLaunch cl = conv2d_launch_shape(d, io->batch, io->height, io->width);
   cl.xhat_in = io->x16; cl.wpk = packed;
-  cl.epi = 1;
   cl.enc_shift = io->shift; cl.enc_act = io->act; cl.enc_slope = io->act == 1 ? io->slope : nullptr;
   cl.enc_slope0 = io->slope0;
   cl.enc_residual = io->residual16;
@@ -62,6 +68,16 @@ int hf_conv2d_forward(const hf_conv2d_desc* d, const void* packed, const hf_conv
   cl.enc_s2 = io->y16b_scale; cl.enc_b2 = io->y16b_shift; cl.enc_y16b = io->y16b;
   cl.out_nchw = io->y32_nchw;
   return launch_conv(cl, (cudaStream_t)stream, nullptr);
+}
+
+int hf_conv2d_plan_query(const hf_conv2d_desc* d, int batch, int height, int width, int* out) {
+  int rc = check_conv2d(d);
+  if (rc) return rc;
+  HF_REQUIRE(out, "hf_conv2d_plan_query: null output");
+  ConvPlan pl;
+  if ((rc = conv_plan(conv2d_launch_shape(d, batch, height, width), &pl))) return rc;
+  conv_plan_export(pl, out);
+  return HF_OK;
 }
 
 int hf_nchw_to_nhwc16(const float* x, const float* scale, const float* shift, void* y16, int batch, int channels,

@@ -114,7 +114,6 @@ struct ConvLaunch {
   const float* rgb_w;     // [3,Cout] (pre-scaled 1/sqrt(Cout)) or NULL
   const float* rgb_s;     // [B,Cout] ToRGB modulation
   float* rgb_partial;     // [num_n_tiles][B,3,Ho,Wo]
-  int force_n_tile;       // 0 = auto
   // ---- plain (encoder) convolution: epi = 1 selects the affine / PReLU / residual epilogue
   int epi;                // 0 generator epilogue, 1 encoder epilogue
   int stride;             // 1 or 2 (0 = 1)
@@ -131,13 +130,14 @@ struct ConvLaunch {
   void* enc_y16b;
 };
 struct ConvPlan {
-  // halo, G, na_slots, pitch, b_resident: fields of the plan query ABI (hf_conv_plan_query) that described the
-  // resident-halo scheduler of the B200 kernel this one replaced; conv_wgmma_kernel has no such scheduler and always
-  // reports 0 / 1 / 0 / 0 / 0.  The column-shift boxes below are a different scheme and do not use them.
+  // halo, G, pitch, b_resident: fields of the plan query ABI (hf_conv_plan_query) that described the resident-halo
+  // scheduler of the B200 kernel this one replaced; conv_wgmma_kernel has no such scheduler and always reports
+  // 0 / 1 / 0 / 0.
   int halo;
   int G;
   int ng;                 // consumer warpgroups (MMA + epilogue), 64 GEMM rows each
-  int na_slots, pitch;
+  int na_slots;           // activation ring slots: kShiftASlots with shift_boxes, 0 on the per-tap path
+  int pitch;
   int b_resident;
   // 1: one (TH + 2)-row activation box per (channel chunk, column shift) serves the three row shifts; activation
   // boxes and weight boxes then have separate rings (kShiftASlots slots of a_slot_bytes; `stages` weight slots)
@@ -152,6 +152,7 @@ struct ConvPlan {
   int num_tiles, grid;
 };
 int conv_plan(const ConvLaunch& a, ConvPlan* p);
+void conv_plan_export(const ConvPlan& pl, int* out /* host[12], the layout of hf_conv_plan_query */);
 int conv_up_nc(int Cout);            // couts per N tile used when packing an upsampling conv
 int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out);
 

@@ -105,8 +105,11 @@ typedef struct {
 size_t hf_conv_workspace_bytes(const hf_conv_desc* d, int batch, int height, int width);
 
 /* Introspection (tests / DESIGN tables; needs no device): the tiling the library will use for this
- * conv.  out[12] = {halo kernel?, n_tile, num_n_tiles, tiles per round G, halo ring slots, halo pitch,
- * weights resident?, pipeline stages, dynamic smem bytes, work items, grid, channels per K chunk}. */
+ * conv.  out[12] = {0, n_tile, num_n_tiles, 1, activation ring slots, 0, 0, pipeline stages, dynamic smem bytes,
+ * work items (M tiles x N tiles), grid, channels per K chunk}.  out[4] tells the two mainloops apart: the slot count
+ * of the activation ring on the column-shift path (stride-1 3x3 on 16 x 8 tiles of one sample), 0 on the per-tap
+ * path, whose activation boxes share the ring slots of the weight boxes.  out[0], out[3], out[5] and out[6] are
+ * constants kept for callers of the earlier layout. */
 int hf_conv_plan_query(const hf_conv_desc* d, int batch, int height, int width, int* out /* host[12] */);
 
 /* Replaces ModulatedConv2d.forward (model.py:238-279) / StyledConv.forward (model.py:337-343). */
@@ -230,6 +233,9 @@ typedef struct {
 
 /* Replaces nn.Conv2d.forward (+ the folded BatchNorm2d / PReLU / LeakyReLU / residual add around it). */
 int hf_conv2d_forward(const hf_conv2d_desc* d, const void* packed, const hf_conv2d_io* io, void* stream);
+
+/* hf_conv_plan_query for the launch hf_conv2d_forward makes at this input size (needs no device): same out[12]. */
+int hf_conv2d_plan_query(const hf_conv2d_desc* d, int batch, int height, int width, int* out /* host[12] */);
 
 /* x [B,C,H,W] fp32 NCHW -> y16 [B,H,W,c_pad] 16-bit NHWC, y = x*scale[c] + shift[c] (NULL = identity), zero padded */
 int hf_nchw_to_nhwc16(const float* x, const float* scale, const float* shift, void* y16, int batch, int channels,

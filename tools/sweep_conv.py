@@ -41,5 +41,5 @@ for (cin, cout, r, up) in LAYERS:
         lib.hf_conv_plan_query(C.byref(desc), B, r, r, plan)
         gf = 2.0 * cin * cout * 9 * r * r * B / 1e9
         print(f"{cin:4d}->{cout:4d} r={r:4d} up={up} B={B:3d}  {ms.value * 1e3:8.1f} us  {gf / ms.value:8.1f} TFLOP/s alg"
-              f"  plan(halo,n_tile,n_n,G,na,pitch,res,stages,smem,work,grid,kc)={list(plan)}", flush=True)
+              f"  plan(0,n_tile,n_n,1,a_slots,0,0,stages,smem,work,grid,kc)={list(plan)}", flush=True)
         del x, y, ws
