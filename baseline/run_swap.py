@@ -1,11 +1,13 @@
 """One process = one arm of the full `HairFast.swap()` comparison (BASELINE configs[2], SURVEY 8d config 3).
 
-    python baseline/run_swap.py --mode reference|overlay|overlay_fast|overlay_sean --work DIR --out result.pt [--reps N]
+    python baseline/run_swap.py --mode reference|overlay|overlay_fast|overlay_sean|overlay_sean_full --work DIR
+                                --out result.pt [--reps N]
 
 * reference     the unmodified reference (oracle/_ref): cuDNN grouped convolutions + its two JIT kernels, fp32/TF32
 * overlay       the same checkout with hairfastgan_b200.install() active (this package's modules under its names)
 * overlay_fast  overlay + install(skip_fse_reconstruction=True) (hairfastgan_b200/fse_fast.py)
 * overlay_sean  overlay + install(sean=True): SEAN's decode_sean on hairfastgan_b200/sean.py
+* overlay_sean_full  overlay + install(sean=True, sean_encode=True): SEAN's encode_sean and decode_sean on it
 
 Three synthetic images `torch.rand(3,1024,1024)` (seeds 0,1,2) are passed as tensors (hair_swap.py:63-105), synthetic
 checkpoints come from baseline/synth_checkpoints.py, `swap(..., seed=3407)` is the default seed (utils/seed.py:22-28).
@@ -29,7 +31,8 @@ from baseline import refenv, synth_checkpoints  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--mode", choices=["reference", "overlay", "overlay_fast", "overlay_sean"], required=True)
+    ap.add_argument("--mode", choices=["reference", "overlay", "overlay_fast", "overlay_sean", "overlay_sean_full"],
+                    required=True)
     ap.add_argument("--work", default="/tmp/hairfast_work")
     ap.add_argument("--out", default=None)
     ap.add_argument("--reps", type=int, default=2)
@@ -44,8 +47,9 @@ def main():
         import subprocess
         subprocess.run([sys.executable, os.path.join(HERE, "synth_checkpoints.py"), work], check=True)
 
+    sean = {"overlay_sean": {"sean": True}, "overlay_sean_full": {"sean": True, "sean_encode": True}}.get(a.mode, {})
     refenv.activate(overlay=a.mode != "reference", skip_fse_reconstruction=a.mode == "overlay_fast", workdir=work,
-                    **({"sean": True} if a.mode == "overlay_sean" else {}))
+                    **sean)
     import torch
     assert torch.cuda.is_available(), "run_swap.py needs a GPU (tools/dryrun_swap_cpu.py is the CPU dry run)"
     from hair_swap import HairFast, get_parser      # the reference's own hair_swap.py

@@ -34,7 +34,7 @@ class hf_conv_io(C.Structure):
 
 class hf_conv2d_desc(C.Structure):
     _fields_ = [("cin", C.c_int), ("cout", C.c_int), ("cin_pad", C.c_int), ("ksize", C.c_int), ("stride", C.c_int),
-                ("groups", C.c_int), ("dtype", C.c_int)]
+                ("groups", C.c_int), ("dtype", C.c_int), ("prepadded", C.c_int), ("transposed", C.c_int)]
 
 
 class hf_conv2d_io(C.Structure):
@@ -107,6 +107,11 @@ SYMBOLS = {
                                     C.c_int, C.c_int, C.c_void_p]),
     "hf_nhwc16_to_nchw": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "hf_channel_reduce_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "hf_instance_norm_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "hf_instance_norm_lrelu_nhwc16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float,
+                                                C.c_int, C.c_void_p]),
+    "hf_reflect_pad1_nhwc16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                         C.c_void_p]),
     "hf_channel_mean_nhwc16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                          C.c_void_p]),
     "hf_se_gate_nhwc16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
@@ -144,6 +149,8 @@ SYMBOLS = {
     "hf_sean_style_tables": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(hf_sean_ace_tables), C.c_int, C.c_void_p,
                                        C.c_void_p]),
     "hf_sean_ace_apply": (C.c_int, [C.c_void_p] * 8 + [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "hf_sean_class_means": (C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                      C.c_void_p]),
     "hf_sean_conv_img": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                    C.c_void_p]),
     "hf_generator_packed_bytes":(C.c_size_t, [C.POINTER(hf_gen_config)]),

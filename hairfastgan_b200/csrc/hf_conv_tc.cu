@@ -45,6 +45,7 @@ struct ConvKernelParams {
   int B, H, W, Cin, Cout;
   int Ho, Wo;
   int taps, up, act;
+  int pad;                 // input rows / columns the taps reach above / left of an output pixel (0: prepadded input)
   int TW, TH, TB, tiles_x, tiles_y;
   int n_tile, num_n_tiles, num_tiles;   // num_tiles = work items (M tiles x N tiles)
   int num_m_tiles;
@@ -243,26 +244,32 @@ __device__ __forceinline__ void load_acc_chunk(const float* srow, int q, uint32_
 // (reference: bottleneck_IR_SE / IBasicBlock conv stacks, encoder4editing/models/encoders/helpers.py:98-120,
 //  FeatureStyleEncoder/arcface/iresnet.py:28-57; GradualStyleBlock psp_encoders.py:34-55)
 // Chunks q0, q0 + 2, ... of the pixel's row.
+// Transposed conv (p.up): chunk q holds output parity q & 3 of channels [(n0 >> 2) + (q >> 2) * 32, + 32) at input
+// pixel (y, x); it is stored at output pixel (2y + parity / 2, 2x + parity % 2).
 template <int DT>
 __device__ __forceinline__ void epilogue_tile_enc(const ConvKernelParams& p, const TableEntry* trow, const float* srow,
                                                   int q0, int n0, int b, int y, int x, bool valid) {
   const int chunks = p.n_tile / 32;
   const size_t plane_o = (size_t)p.Ho * p.Wo;
-  const size_t pix = valid ? ((size_t)b * p.Ho + y) * p.Wo + x : 0;
   const uint32_t trow_s = smem_u32(trow);
   const int variant = p.out_nchw ? 3 : ((p.enc_residual ? 1 : 0) | (p.enc_y16b ? 2 : 0));
   const bool post = p.enc_post != 0;
   for (int q = q0; q < chunks; q += 2) {
     uint32_t acc[32];
     load_acc_chunk(srow, q, acc);
-    const int o_base = n0 + q * 32;
+    const int par = p.up ? (q & 3) : 0;
+    const int t_base = p.up ? (q >> 2) * 32 : q * 32;          // channel offset inside the tile
+    const int o_base = (p.up ? (n0 >> 2) : n0) + t_base;
+    const int yo = p.up ? 2 * y + (par >> 1) : y;
+    const int xo = p.up ? 2 * x + (par & 1) : x;
+    const size_t pix = valid ? ((size_t)b * p.Ho + yo) * p.Wo + xo : 0;
     const size_t eo = pix * p.Cout + o_base;
     const uint4* res = (p.enc_residual && valid) ? reinterpret_cast<const uint4*>(p.enc_residual + eo) : nullptr;
     uint4* dst = (p.xhat_out && valid) ? reinterpret_cast<uint4*>(p.xhat_out + eo) : nullptr;
     uint4* dst_b = (p.enc_y16b && valid) ? reinterpret_cast<uint4*>(p.enc_y16b + eo) : nullptr;
-    float* onchw = (p.out_nchw && valid) ? p.out_nchw + ((size_t)b * p.Cout + o_base) * plane_o + (size_t)y * p.Wo + x
+    float* onchw = (p.out_nchw && valid) ? p.out_nchw + ((size_t)b * p.Cout + o_base) * plane_o + (size_t)yo * p.Wo + xo
                                          : nullptr;
-    const uint32_t ts = trow_s + (uint32_t)(q * 32) * (uint32_t)sizeof(TableEntry);
+    const uint32_t ts = trow_s + (uint32_t)t_base * (uint32_t)sizeof(TableEntry);
     switch (variant) {       // uniform across the CTA
       case 0: epi_chunk_enc<DT, false, false, false>(ts, acc, res, dst, dst_b, onchw, plane_o, post); break;
       case 1: epi_chunk_enc<DT, true, false, false>(ts, acc, res, dst, dst_b, onchw, plane_o, post); break;
@@ -420,7 +427,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       uint32_t phase = 0;
       int a_stage = 0;
       uint32_t a_phase = 0;
-      const int pad = (p.taps == 9) ? 1 : 0;
+      const int pad = p.pad;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         const int nt = tile % p.num_n_tiles;
         const MTile tc = decode_mtile(p, tile / p.num_n_tiles);
@@ -433,7 +440,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               mbar_wait_nocall(&a_empty_bar[a_stage], a_phase ^ 1);
               mbar_expect_tx(&a_full_bar[a_stage], p.a_slot_bytes);
               tma_load_4d(a_ring + (size_t)a_stage * p.a_slot_bytes, &tmA, &a_full_bar[a_stage],
-                          c_off + kc * KCHUNK, tc.x0 + dx - 1, tc.y0 - 1, b0);
+                          c_off + kc * KCHUNK, tc.x0 + dx - pad, tc.y0 - pad, b0);
               if (++a_stage == kShiftASlots) { a_stage = 0; a_phase ^= 1; }
               for (int dy = 0; dy < 3; ++dy) {
                 mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
@@ -596,8 +603,12 @@ int conv_plan(const ConvLaunch& a, ConvPlan* p) {
   HF_REQUIRE(a.Cout % 32 == 0 && a.Cout >= 32, "conv: Cout=%d must be a multiple of 32", a.Cout);
   HF_REQUIRE(!a.up || a.taps == 9, "conv: upsample needs a 3x3 kernel");
   HF_REQUIRE(stride == 1 || (a.H % 2 == 0 && a.W % 2 == 0) || (a.H == 1 && a.W == 1), "conv: stride 2 needs even H, W");
-  // the GEMM rows are OUTPUT pixels (input pixels for the polyphase up-conv)
-  const int MH = stride == 2 ? (a.H + 1) / 2 : a.H, MW = stride == 2 ? (a.W + 1) / 2 : a.W;
+  HF_REQUIRE(!a.prepadded || (a.taps == 9 && stride == 1 && !a.up && a.H > 2 && a.W > 2),
+             "conv: a prepadded input needs a stride-1 3x3 conv and H, W > 2");
+  // the GEMM rows are OUTPUT pixels (input pixels for the polyphase up-conv); a prepadded input carries a 1-pixel
+  // border that yields no output pixel
+  const int MH = stride == 2 ? (a.H + 1) / 2 : a.H - (a.prepadded ? 2 : 0);
+  const int MW = stride == 2 ? (a.W + 1) / 2 : a.W - (a.prepadded ? 2 : 0);
   p->halo = 0; p->G = 1; p->na_slots = 0; p->pitch = 0; p->b_resident = 0; p->a_slot_bytes = 0; p->ng = 2;
   p->TW = MW < 16 ? MW : 16;
   HF_REQUIRE(128 % p->TW == 0, "conv: width %d unsupported (tile width must divide 128)", MW);
@@ -708,9 +719,10 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
   ConvKernelParams kp;
   memset(&kp, 0, sizeof(kp));
   kp.B = a.B; kp.H = a.H; kp.W = a.W; kp.Cin = a.Cin; kp.Cout = a.Cout;
-  kp.Ho = a.up ? 2 * a.H : (stride == 2 ? (a.H + 1) / 2 : a.H);
-  kp.Wo = a.up ? 2 * a.W : (stride == 2 ? (a.W + 1) / 2 : a.W);
+  kp.Ho = a.up ? 2 * a.H : (stride == 2 ? (a.H + 1) / 2 : a.H - (a.prepadded ? 2 : 0));
+  kp.Wo = a.up ? 2 * a.W : (stride == 2 ? (a.W + 1) / 2 : a.W - (a.prepadded ? 2 : 0));
   kp.taps = a.taps; kp.up = a.up; kp.act = a.act;
+  kp.pad = (a.taps == 9 && !a.prepadded) ? 1 : 0;
   kp.TW = pl.TW; kp.TH = pl.TH; kp.TB = pl.TB; kp.tiles_x = pl.tiles_x; kp.tiles_y = pl.tiles_y;
   kp.n_tile = pl.n_tile; kp.num_n_tiles = pl.num_n_tiles; kp.num_tiles = pl.num_tiles;
   kp.num_m_tiles = pl.num_m_tiles;
@@ -740,7 +752,6 @@ int launch_conv(const ConvLaunch& a, cudaStream_t st, ConvPlan* plan_out) {
   kp.enc_s2 = a.enc_s2; kp.enc_b2 = a.enc_b2;
   kp.enc_residual = (const uint16_t*)a.enc_residual;
   kp.enc_y16b = (uint16_t*)a.enc_y16b;
-  HF_REQUIRE(!a.epi || !a.up, "conv: the encoder epilogue has no upsampling form");
   if (plan_out) *plan_out = pl;
 
   const bool bf = a.dtype == HF_BF16;

@@ -18,6 +18,12 @@ static int check_conv2d(const hf_conv2d_desc* d) {
              "conv2d: cin_pad=%d must be >= cin and a multiple of 32 per group", d->cin_pad);
   HF_REQUIRE(d->groups == 1 || d->cin_pad == d->cin, "conv2d: channel padding is not supported with groups > 1");
   HF_REQUIRE(d->cout % 32 == 0, "conv2d: cout=%d must be a multiple of 32", d->cout);
+  HF_REQUIRE((d->prepadded == 0 || d->prepadded == 1) && (d->transposed == 0 || d->transposed == 1),
+             "conv2d: prepadded / transposed must be 0 or 1");
+  HF_REQUIRE(!d->prepadded || (d->ksize == 3 && d->stride == 1 && !d->transposed),
+             "conv2d: a prepadded input needs a stride-1 3x3 conv");
+  HF_REQUIRE(!d->transposed || (d->ksize == 3 && d->stride == 2 && d->groups == 1),
+             "conv2d: the transposed form is ConvTranspose2d(3, stride 2, padding 1, output_padding 1), no groups");
   return HF_OK;
 }
 
@@ -28,7 +34,8 @@ static ConvLaunch conv2d_launch_shape(const hf_conv2d_desc* d, int batch, int he
   cl.B = batch; cl.H = height; cl.W = width;
   cl.Cin = d->cin_pad; cl.Cout = d->cout;
   cl.taps = d->ksize * d->ksize; cl.dtype = d->dtype;
-  cl.stride = d->stride; cl.groups = d->groups;
+  cl.stride = d->transposed ? 1 : d->stride; cl.groups = d->groups;   // transposed: the four-parity 3x3 form
+  cl.up = d->transposed; cl.prepadded = d->prepadded;
   cl.epi = 1;
   return cl;
 }
@@ -37,7 +44,7 @@ extern "C" {
 
 size_t hf_conv2d_packed_bytes(const hf_conv2d_desc* d) {
   if (check_conv2d(d)) return 0;
-  return align256((size_t)d->cout * d->ksize * d->ksize * (d->cin_pad / d->groups) * 2);
+  return align256((size_t)(d->transposed ? 4 : 1) * d->cout * d->ksize * d->ksize * (d->cin_pad / d->groups) * 2);
 }
 
 int hf_conv2d_pack(const hf_conv2d_desc* d, const float* weight, const float* out_scale, void* packed, void* stream) {
@@ -45,6 +52,9 @@ int hf_conv2d_pack(const hf_conv2d_desc* d, const float* weight, const float* ou
   if (rc) return rc;
   if ((rc = ensure_device_current())) return rc;
   HF_REQUIRE(weight && packed && ((uintptr_t)packed & 255) == 0, "hf_conv2d_pack: null / unaligned pointer");
+  if (d->transposed)
+    return launch_pack_conv2d_transposed(weight, out_scale, packed, d->cout, d->cin, d->cin_pad, d->dtype,
+                                         (cudaStream_t)stream);
   return launch_pack_conv2d(weight, out_scale, packed, d->cout, d->cin / d->groups, d->cin_pad / d->groups, d->ksize,
                             d->dtype, (cudaStream_t)stream);
 }
@@ -98,6 +108,26 @@ int hf_nhwc16_to_nchw(const void* x16, float* y, int batch, int channels, int he
 size_t hf_channel_reduce_workspace_bytes(int batch, int hw, int channels) {
   if (batch <= 0 || hw <= 0 || channels <= 0) return 0;
   return (size_t)batch * channel_reduce_splits(batch, hw, channels) * channels * sizeof(float);
+}
+
+size_t hf_instance_norm_workspace_bytes(int batch, int hw, int channels) {
+  if (batch <= 0 || hw <= 0 || channels <= 0) return 0;
+  return hf_channel_reduce_workspace_bytes(batch, hw, channels) + 2 * (size_t)batch * channels * sizeof(float);
+}
+
+int hf_instance_norm_lrelu_nhwc16(const void* x16, void* y16, void* workspace, int batch, int hw, int channels,
+                                  float slope, int dtype, void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  return launch_instance_norm_act(x16, y16, (float*)workspace, batch, hw, channels, 1e-5f, slope, dtype,
+                                  (cudaStream_t)stream);
+}
+
+int hf_reflect_pad1_nhwc16(const void* x16, void* y16, int batch, int height, int width, int channels, int dtype,
+                           void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  return launch_reflect_pad1(x16, y16, batch, height, width, channels, dtype, (cudaStream_t)stream);
 }
 
 int hf_channel_mean_nhwc16(const void* x16, float* mean, void* workspace, int batch, int hw, int channels, int dtype,

@@ -12,6 +12,16 @@ static inline int cdiv_i(int64_t a, int64_t b) { return (int)((a + b - 1) / b); 
 template <int DT>
 __device__ __forceinline__ float ld16(const uint16_t* p) { return Half2T<DT>::to_float(*p); }
 
+template <int DT>
+__device__ __forceinline__ void unpack8(const uint4& v, float* f) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    f[2 * k] = Half2T<DT>::to_float((uint16_t)(w[k] & 0xFFFF));
+    f[2 * k + 1] = Half2T<DT>::to_float((uint16_t)(w[k] >> 16));
+  }
+}
+
 // wpk[o][tap*cin_pad + c] = w[o, c, tap] * out_scale[o]   (c >= cin -> 0: channel padding of the input)
 template <int DT>
 __global__ void __launch_bounds__(256) pack_conv2d_kernel(const float* __restrict__ w, const float* __restrict__ osc,
@@ -26,6 +36,48 @@ __global__ void __launch_bounds__(256) pack_conv2d_kernel(const float* __restric
     const float v = c < cin_g ? w[((size_t)o * cin_g + c) * taps + t] * sc : 0.f;
     wpk[(size_t)o * K + (size_t)t * cin_pad + c] = Half2T<DT>::one(v);
   }
+}
+
+// ConvTranspose2d(3, stride 2, padding 1, output_padding 1) as four 3x3 correlations over the input with padding 1,
+// one per output parity (a, b) = (yo % 2, xo % 2), stacked along N (row (o / 32) * 128 + (2a + b) * 32 + o % 32, the
+// layout of the generator's upsampling conv, DESIGN section 3).  Output 2m takes kernel row 1 at input m; output
+// 2m + 1 takes kernel row 2 at input m and kernel row 0 at input m + 1 (the zero fill gives input H), so the tap
+// (dy, dx) of parity (a, b) is w[c, o, ky, kx] with ky = {a = 0: dy 1 -> 1; a = 1: dy 1 -> 2, dy 2 -> 0}, same for kx.
+__device__ __forceinline__ int transposed_k(int parity, int d) {
+  return parity == 0 ? (d == 1 ? 1 : -1) : (d == 1 ? 2 : (d == 2 ? 0 : -1));
+}
+
+template <int DT>
+__global__ void __launch_bounds__(256) pack_conv2d_transposed_kernel(const float* __restrict__ w,
+                                                                     const float* __restrict__ osc,
+                                                                     uint16_t* __restrict__ wpk, int cout, int cin,
+                                                                     int cin_pad) {
+  const int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)4 * cout * cin_pad) return;
+  const int c = (int)(idx % cin_pad), n = (int)(idx / cin_pad);
+  const int par = (n & 127) >> 5, o = (n >> 7) * 32 + (n & 31);
+  const float sc = osc ? osc[o] : 1.f;
+  const size_t K = (size_t)9 * cin_pad;
+  for (int t = 0; t < 9; ++t) {
+    const int ky = transposed_k(par >> 1, t / 3), kx = transposed_k(par & 1, t % 3);
+    const float v = (c < cin && ky >= 0 && kx >= 0) ? w[(((size_t)c * cout + o) * 3 + ky) * 3 + kx] * sc : 0.f;
+    wpk[(size_t)n * K + (size_t)t * cin_pad + c] = Half2T<DT>::one(v);
+  }
+}
+
+int launch_pack_conv2d_transposed(const float* w, const float* out_scale, void* wpk, int cout, int cin, int cin_pad,
+                                  int dtype, cudaStream_t st) {
+  HF_REQUIRE(w && wpk, "pack_conv2d_transposed: null pointer");
+  HF_REQUIRE(cout % 32 == 0 && cin_pad >= cin && cin_pad % 32 == 0, "pack_conv2d_transposed: bad channels %d -> %d",
+             cin, cout);
+  const int grid = cdiv_i((int64_t)4 * cout * cin_pad, 256);
+  if (dtype == HF_BF16)
+    pack_conv2d_transposed_kernel<HF_BF16><<<grid, 256, 0, st>>>(w, out_scale, (uint16_t*)wpk, cout, cin, cin_pad);
+  else
+    pack_conv2d_transposed_kernel<HF_F16><<<grid, 256, 0, st>>>(w, out_scale, (uint16_t*)wpk, cout, cin, cin_pad);
+  HF_LAUNCH_OK("pack_conv2d_transposed");
+  count_launch();
+  return HF_OK;
 }
 
 int launch_pack_conv2d(const float* w, const float* out_scale, void* wpk, int cout, int cin_g, int cin_pad, int ksize,
@@ -121,8 +173,10 @@ int launch_nhwc16_to_nchw(const void* x16, float* y, int B, int C, int HW, int d
 // Squeeze-excite pooling (SEModule, helpers.py:57-75) in two deterministic stages.
 // Stage 1: per-(b, pixel split, 64-channel slab) partial sums of an NHWC 16-bit tensor.  256 threads = 8 lanes of
 // 8 channels (16-byte loads) x 32 pixel rows; fixed summation order.  part[(b*S + s)*C + c].
-template <int DT>
+// CENTER: partial sums of (x - center[b, c])^2 instead (the second pass of the instance-norm variance).
+template <int DT, bool CENTER>
 __global__ void __launch_bounds__(256) channel_sum_partial_kernel(const uint16_t* __restrict__ x,
+                                                                  const float* __restrict__ center,
                                                                   float* __restrict__ part, int HW, int C, int chunk) {
   __shared__ float red[32][65];
   const int b = blockIdx.y, s = blockIdx.z, S = gridDim.z, c0 = blockIdx.x * 64;
@@ -131,13 +185,23 @@ __global__ void __launch_bounds__(256) channel_sum_partial_kernel(const uint16_t
   float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   const int p0 = s * chunk, p1 = min(HW, p0 + chunk);
   if (c < C) {
+    float m[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) m[k] = CENTER ? __ldg(center + (size_t)b * C + c + k) : 0.f;
     for (int p = p0 + row; p < p1; p += 32) {
       const uint4 v = __ldg(reinterpret_cast<const uint4*>(x + ((size_t)b * HW + p) * C + c));
       const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        acc[2 * k] += Half2T<DT>::to_float((uint16_t)(w[k] & 0xFFFF));
-        acc[2 * k + 1] += Half2T<DT>::to_float((uint16_t)(w[k] >> 16));
+        const float lo = Half2T<DT>::to_float((uint16_t)(w[k] & 0xFFFF)), hi = Half2T<DT>::to_float((uint16_t)(w[k] >> 16));
+        if (CENTER) {
+          const float dl = lo - m[2 * k], dh = hi - m[2 * k + 1];
+          acc[2 * k] = fmaf(dl, dl, acc[2 * k]);
+          acc[2 * k + 1] = fmaf(dh, dh, acc[2 * k + 1]);
+        } else {
+          acc[2 * k] += lo;
+          acc[2 * k + 1] += hi;
+        }
       }
     }
   }
@@ -208,18 +272,120 @@ int launch_se_gate(const void* x16, const float* fc1, const float* fc2, float* o
   return HF_OK;
 }
 
-// stage 1 alone: ws[(b*S + s)*C + c] = partial channel sums; *splits = S
-int launch_channel_partial(const void* x16, float* ws, int B, int HW, int C, int dtype, cudaStream_t st, int* splits) {
+// stage 1 alone: ws[(b*S + s)*C + c] = partial channel sums (of (x - center)^2 with a center); *splits = S
+static int channel_partial(const void* x16, const float* center, float* ws, int B, int HW, int C, int dtype,
+                           cudaStream_t st, int* splits) {
   HF_REQUIRE(x16 && ws && C % 8 == 0 && B > 0 && HW > 0, "channel_partial: bad arguments");
   const int S = channel_reduce_splits(B, HW, C), chunk = cdiv_i(HW, S);
   dim3 grid(cdiv_i(C, 64), B, S);
-  if (dtype == HF_BF16)
-    channel_sum_partial_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, ws, HW, C, chunk);
-  else
-    channel_sum_partial_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, ws, HW, C, chunk);
+  const uint16_t* x = (const uint16_t*)x16;
+  if (center) {
+    if (dtype == HF_BF16)
+      channel_sum_partial_kernel<HF_BF16, true><<<grid, 256, 0, st>>>(x, center, ws, HW, C, chunk);
+    else
+      channel_sum_partial_kernel<HF_F16, true><<<grid, 256, 0, st>>>(x, center, ws, HW, C, chunk);
+  } else {
+    if (dtype == HF_BF16)
+      channel_sum_partial_kernel<HF_BF16, false><<<grid, 256, 0, st>>>(x, nullptr, ws, HW, C, chunk);
+    else
+      channel_sum_partial_kernel<HF_F16, false><<<grid, 256, 0, st>>>(x, nullptr, ws, HW, C, chunk);
+  }
   HF_LAUNCH_OK("channel_sum_partial");
   count_launch();
   if (splits) *splits = S;
+  return HF_OK;
+}
+
+int launch_channel_partial(const void* x16, float* ws, int B, int HW, int C, int dtype, cudaStream_t st, int* splits) {
+  return channel_partial(x16, nullptr, ws, B, HW, C, dtype, st, splits);
+}
+
+// y = act((x - mean[b,c]) * rsqrt(var[b,c] + eps)), act = LeakyReLU(slope); 8 channels (16 bytes) per thread
+template <int DT>
+__global__ void __launch_bounds__(256) instance_norm_apply_kernel(const uint16_t* __restrict__ x,
+                                                                  const float* __restrict__ mean,
+                                                                  const float* __restrict__ var,
+                                                                  uint16_t* __restrict__ y, int HW, int C8, float eps,
+                                                                  float slope, int total8) {
+  const int C = C8 * 8;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total8; i += gridDim.x * blockDim.x) {
+    const int c = (i % C8) * 8, b = i / C8 / HW;
+    float v[8];
+    unpack8<DT>(__ldg(reinterpret_cast<const uint4*>(x + (size_t)i * 8)), v);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const size_t bc = (size_t)b * C + c + k;
+      const float t = (v[k] - __ldg(mean + bc)) * rsqrtf(__ldg(var + bc) + eps);
+      v[k] = t > 0.f ? t : t * slope;
+    }
+    uint4 o;
+    o.x = Half2T<DT>::pack(v[0], v[1]); o.y = Half2T<DT>::pack(v[2], v[3]);
+    o.z = Half2T<DT>::pack(v[4], v[5]); o.w = Half2T<DT>::pack(v[6], v[7]);
+    *reinterpret_cast<uint4*>(y + (size_t)i * 8) = o;
+  }
+}
+
+// InstanceNorm2d(affine=False): mean = the channel mean of launch_se_gate's two stages; var = the same two stages over
+// (x - mean)^2 (no E[x^2] - E[x]^2 cancellation); then the normalisation + LeakyReLU.  ws = [partials | mean | var].
+int launch_instance_norm_act(const void* x16, void* y16, float* ws, int B, int HW, int C, float eps, float slope,
+                             int dtype, cudaStream_t st) {
+  HF_REQUIRE(x16 && y16 && ws, "instance_norm: null pointer");
+  HF_REQUIRE(B > 0 && HW > 0 && C > 0 && C % 8 == 0, "instance_norm: bad shape B=%d HW=%d C=%d (C %% 8)", B, HW, C);
+  const int64_t total8 = (int64_t)B * HW * C / 8;
+  HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch",
+             (long long)total8);
+  const int S = channel_reduce_splits(B, HW, C);
+  float* mean = ws + (size_t)B * S * C;
+  float* var = mean + (size_t)B * C;
+  int rc = channel_partial(x16, nullptr, ws, B, HW, C, dtype, st, nullptr);
+  if (rc) return rc;
+  se_gate_kernel<<<B, 256, (size_t)C * sizeof(float), st>>>(ws, S, 1.f / (float)HW, nullptr, nullptr, mean, C, 0);
+  HF_LAUNCH_OK("instance_norm_mean");
+  if ((rc = channel_partial(x16, mean, ws, B, HW, C, dtype, st, nullptr))) return rc;
+  se_gate_kernel<<<B, 256, (size_t)C * sizeof(float), st>>>(ws, S, 1.f / (float)HW, nullptr, nullptr, var, C, 0);
+  HF_LAUNCH_OK("instance_norm_var");
+  const int grid = (int)std::min<int64_t>((total8 + 255) / 256, (int64_t)num_sms() * 16);
+  if (dtype == HF_BF16)
+    instance_norm_apply_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, mean, var, (uint16_t*)y16, HW,
+                                                              C / 8, eps, slope, (int)total8);
+  else
+    instance_norm_apply_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, mean, var, (uint16_t*)y16, HW,
+                                                             C / 8, eps, slope, (int)total8);
+  HF_LAUNCH_OK("instance_norm_apply");
+  count_launch(3);
+  return HF_OK;
+}
+
+// ReflectionPad2d(1): row / column -1 -> 1, H -> H - 2; 8 channels (16 bytes) per thread
+__global__ void __launch_bounds__(256) reflect_pad1_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int H,
+                                                           int W, int C8, int total8) {
+  const int Wp = W + 2, Hp = H + 2;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total8; i += gridDim.x * blockDim.x) {
+    const int c = i % C8;
+    int t = i / C8;
+    const int xo = t % Wp; t /= Wp;
+    const int yo = t % Hp;
+    const int b = t / Hp;
+    int yi = yo - 1, xi = xo - 1;
+    yi = yi < 0 ? 1 : (yi >= H ? H - 2 : yi);
+    xi = xi < 0 ? 1 : (xi >= W ? W - 2 : xi);
+    y[i] = __ldg(x + (((size_t)b * H + yi) * W + xi) * C8 + c);
+  }
+}
+
+int launch_reflect_pad1(const void* x16, void* y16, int B, int H, int W, int C, int dtype, cudaStream_t st) {
+  (void)dtype;                                   // a copy: the same kernel for both 16-bit types
+  HF_REQUIRE(x16 && y16, "reflect_pad1: null pointer");
+  HF_REQUIRE(B > 0 && H >= 2 && W >= 2 && C > 0 && C % 8 == 0, "reflect_pad1: bad shape %dx%dx%d (H, W >= 2, C %% 8)",
+             H, W, C);
+  HF_REQUIRE((((uintptr_t)x16 | (uintptr_t)y16) & 15) == 0, "reflect_pad1: 16-bit tensors must be 16-byte aligned");
+  const int64_t total8 = (int64_t)B * (H + 2) * (W + 2) * C / 8;
+  HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch",
+             (long long)total8);
+  const int grid = (int)std::min<int64_t>((total8 + 255) / 256, (int64_t)num_sms() * 16);
+  reflect_pad1_kernel<<<grid, 256, 0, st>>>((const uint4*)x16, (uint4*)y16, H, W, C / 8, (int)total8);
+  HF_LAUNCH_OK("reflect_pad1");
+  count_launch();
   return HF_OK;
 }
 
@@ -375,16 +541,6 @@ __global__ void __launch_bounds__(256) upsample_add_kernel(const uint16_t* __res
       v[u] = (1.f - ly) * ((1.f - lx) * a00 + lx * a01) + ly * ((1.f - lx) * a10 + lx * a11) + ld16<DT>(y + e + u);
     }
     *reinterpret_cast<uint32_t*>(out + e) = Half2T<DT>::pack(v[0], v[1]);
-  }
-}
-
-template <int DT>
-__device__ __forceinline__ void unpack8(const uint4& v, float* f) {
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    f[2 * k] = Half2T<DT>::to_float((uint16_t)(w[k] & 0xFFFF));
-    f[2 * k + 1] = Half2T<DT>::to_float((uint16_t)(w[k] >> 16));
   }
 }
 

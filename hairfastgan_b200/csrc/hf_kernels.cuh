@@ -55,6 +55,15 @@ int launch_scale_copy(const float* src, float* dst, int64_t n, float scale, cuda
 // ---- hf_enc_ops.cu : encoder-side glue kernels -------------------------------------------------
 int launch_pack_conv2d(const float* w, const float* out_scale, void* wpk, int cout, int cin_g, int cin_pad, int ksize,
                        int dtype, cudaStream_t st);
+// ConvTranspose2d(3, stride 2, padding 1, output_padding 1) weight [cin, cout, 3, 3] -> the four-parity 3x3 operand
+// [4 * cout][9 * cin_pad] of the upsampling conv (row (o / 32) * 128 + parity * 32 + o % 32)
+int launch_pack_conv2d_transposed(const float* w, const float* out_scale, void* wpk, int cout, int cin, int cin_pad,
+                                  int dtype, cudaStream_t st);
+// InstanceNorm2d(affine=False, eps) + LeakyReLU(slope) of x16 [B,HW,C] -> y16; ws: channel_reduce floats + 2 * B * C
+int launch_instance_norm_act(const void* x16, void* y16, float* ws, int B, int HW, int C, float eps, float slope,
+                             int dtype, cudaStream_t st);
+// ReflectionPad2d(1): x16 [B,H,W,C] -> y16 [B,H+2,W+2,C]
+int launch_reflect_pad1(const void* x16, void* y16, int B, int H, int W, int C, int dtype, cudaStream_t st);
 int launch_nchw_to_nhwc16(const float* x, const float* scale, const float* shift, void* y16, int B, int C, int Cpad,
                           int HW, int dtype, cudaStream_t st);
 int launch_nhwc16_to_nchw(const void* x16, float* y, int B, int C, int HW, int dtype, cudaStream_t st);
@@ -97,6 +106,7 @@ struct ConvLaunch {
   int B, H, W;            // input spatial size
   int Cin, Cout;
   int taps;               // 9 (3x3, pad 1) or 1 (1x1)
+  int prepadded;          // 1: the stored input already carries the 1-pixel border (3x3, stride 1): output (H-2)x(W-2)
   int up;                 // 1: polyphase stride-2 transposed conv + blur -> output 2H x 2W
   int dtype;
   const void* xhat_in;    // [B,H,W,Cin] 16-bit NHWC (already multiplied by this conv's s[b,cin])

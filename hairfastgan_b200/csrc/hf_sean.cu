@@ -257,6 +257,46 @@ __global__ void __launch_bounds__(256) sean_conv_img_kernel(const uint16_t* __re
   for (int o = 0; o < 3; ++o) y[(size_t)o * R * R + p] = tanhf(acc[o]);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Zencoder.forward's tail (architecture.py:177-207): codes[b][j][c] = mean over the class-j pixels of tanh(y[b][c]),
+// 0 where class j has no pixel.  One CTA per (c, b) plane: thread t accumulates pixels t, t + 256, ... into its own
+// column of per-class sums and counts in shared memory, then warp w reduces classes w, w + 8, w + 16 over the 256
+// columns in a fixed order (no atomics: the result does not depend on scheduling).
+// ------------------------------------------------------------------------------------------------
+constexpr int kMeanThreads = 256;
+__global__ void __launch_bounds__(kMeanThreads) sean_class_means_kernel(const float* __restrict__ y,
+                                                                        const int8_t* __restrict__ labels,
+                                                                        long long label_stride,
+                                                                        float* __restrict__ codes, int C, int HW) {
+  __shared__ float ssum[kClasses][kMeanThreads];
+  __shared__ int scnt[kClasses][kMeanThreads];
+  const int c = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  for (int j = 0; j < kClasses; ++j) { ssum[j][tid] = 0.f; scnt[j][tid] = 0; }
+  const float* plane = y + ((size_t)b * C + c) * HW;
+  const int8_t* L = labels + (size_t)b * label_stride;
+  for (int p = tid; p < HW; p += kMeanThreads) {
+    const int j = L[p];
+    if ((unsigned)j < (unsigned)kClasses) {
+      ssum[j][tid] += tanhf(__ldg(plane + p));
+      scnt[j][tid] += 1;
+    }
+  }
+  __syncthreads();
+  const int lane = tid & 31, warp = tid >> 5;
+  for (int j = warp; j < kClasses; j += kMeanThreads / 32) {
+    float s = 0.f;
+    int n = 0;
+#pragma unroll
+    for (int k = 0; k < kMeanThreads / 32; ++k) { s += ssum[j][lane + 32 * k]; n += scnt[j][lane + 32 * k]; }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+      s += __shfl_xor_sync(0xffffffffu, s, o);
+      n += __shfl_xor_sync(0xffffffffu, n, o);
+    }
+    if (lane == 0) codes[((size_t)b * kClasses + j) * C + c] = n > 0 ? s / (float)n : 0.f;
+  }
+}
+
 int grid_for(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, (int64_t)num_sms() * 16); }
 
 }  // namespace
@@ -345,6 +385,20 @@ int hf_sean_ace_apply(const void* x16, const float* noise, const float* noise_va
     sean_ace_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, noise, noise_var, bn_scale, bn_shift,
                                                   gamma_beta, table, labels, lrelu, (uint16_t*)y16, res, channels);
   HF_LAUNCH_OK("sean_ace");
+  count_launch();
+  return HF_OK;
+}
+
+int hf_sean_class_means(const float* y, const int8_t* labels, long long label_stride, float* codes, int batch,
+                        int channels, int hw, void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  HF_REQUIRE(y && labels && codes, "hf_sean_class_means: null pointer");
+  HF_REQUIRE(batch > 0 && batch <= 65535 && channels > 0 && hw > 0 && label_stride >= hw,
+             "hf_sean_class_means: bad shape B=%d C=%d HW=%d label stride %lld", batch, channels, hw, label_stride);
+  sean_class_means_kernel<<<dim3(channels, batch), kMeanThreads, 0, (cudaStream_t)stream>>>(y, labels, label_stride,
+                                                                                           codes, channels, hw);
+  HF_LAUNCH_OK("sean_class_means");
   count_launch();
   return HF_OK;
 }

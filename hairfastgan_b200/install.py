@@ -36,6 +36,8 @@ After ``install()`` the import statements of the reference resolve to this packa
 * opt-in, ``install(sean=True)``: ``decode_sean`` (models/sean_codes/models/pix2pix_model.py:309-325) is rebound inside
   ``models.sean_codes.models.pix2pix_model`` and ``models.Alignment`` (which imports the name, Alignment.py:10)
                                                                                     -> ``hairfastgan_b200.sean``
+* opt-in, ``install(sean_encode=True)``: ``encode_sean`` (pix2pix_model.py:299-306) is rebound in the same two modules
+                                                                                    -> ``hairfastgan_b200.sean``
 
 Nothing in the reference tree is edited and its JIT build of the two 2019 CUDA extensions
 (op/fused_act.py:10-16, op/upfirdn2d.py:10-16) never runs.
@@ -92,29 +94,31 @@ _FSE_TRAINER = "trainer"
 # face parsing: FaceParsing_tensor.parsing_img (my_parsing_util.py:70-89) -> label-only path of hairfastgan_b200/parsing_fast.py
 _PARSING_UTIL = "models.CtrlHair.external_code.face_parsing.my_parsing_util"
 _patched_parsing = []
-# SEAN decode (opt-in): module -> the reference decode_sean it held before the rebind
+# SEAN (opt-in): the function names rebound in these modules, and (module, name) -> the reference function it held
 _SEAN_MODULES = ("models.sean_codes.models.pix2pix_model", "models.Alignment")
+_sean_names = set()
 _sean_saved = {}
 _post_import = set()          # module names the meta-path hook currently patches
 _patched_trainers = []
 
 
-def _patch_sean(module) -> None:
-    ours = importlib.import_module("hairfastgan_b200.sean").decode_sean
-    current = getattr(module, "decode_sean", None)
+def _patch_sean(module, name: str) -> None:
+    ours = getattr(importlib.import_module("hairfastgan_b200.sean"), name)
+    current = getattr(module, name, None)
     if current is None or current is ours:
         # models.Alignment imported the name after pix2pix_model was rebound: restore it to the reference's function
         ref = sys.modules.get(_SEAN_MODULES[0])
-        if current is ours and ref is not None and ref in _sean_saved and module not in _sean_saved:
-            _sean_saved[module] = _sean_saved[ref]
+        if current is ours and ref is not None and (ref, name) in _sean_saved and (module, name) not in _sean_saved:
+            _sean_saved[(module, name)] = _sean_saved[(ref, name)]
         return
-    _sean_saved[module] = current
-    module.decode_sean = ours
+    _sean_saved[(module, name)] = current
+    setattr(module, name, ours)
 
 
 def _patch_postprocess(module) -> None:
     if module.__name__ in _SEAN_MODULES:
-        _patch_sean(module)
+        for name in sorted(_sean_names):
+            _patch_sean(module, name)
         return
     if module.__name__ == _PARSING_UTIL:
         fast = importlib.import_module("hairfastgan_b200.parsing_fast")
@@ -188,12 +192,12 @@ def _register(ref_name: str, ours: str) -> None:
 
 def install(generator: bool = True, encoders: bool = True, postprocess: bool = True, segmentation: bool = True,
             glue: bool = True, skip_fse_reconstruction: bool = False, fuse_face_parsing: bool = True,
-            sean: bool = False) -> None:
+            sean: bool = False, sean_encode: bool = False) -> None:
     """Register the overlay.  ``generator=False`` swaps only the operator package (L1 boundary) and leaves the
     reference's own ``models/stylegan2/model.py`` classes in place on top of our ops; ``encoders=False`` keeps
     the reference's PyTorch encoders; ``postprocess=False`` keeps its PostProcess conv stack; ``segmentation=False``
-    its BiSeNet.  ``sean=True`` (off by default) runs SEAN's ``decode_sean`` on our kernels (``encode_sean`` and the
-    Zencoder stay the reference's)."""
+    its BiSeNet.  ``sean=True`` (off by default) runs SEAN's ``decode_sean`` on our kernels; ``sean_encode=True`` (off
+    by default, independent of ``sean``) runs its ``encode_sean`` (the Zencoder) on them."""
     if segmentation:
         for ref_name, ours in _SEGMENTATION.items():
             _register(ref_name, ours)
@@ -220,6 +224,10 @@ def install(generator: bool = True, encoders: bool = True, postprocess: bool = T
         # reads (x_1_recon comes back as None) and draws the same noise, so later random numbers are unchanged
         _post_import.add(_FSE_TRAINER)
     if sean:
+        _sean_names.add("decode_sean")
+    if sean_encode:
+        _sean_names.add("encode_sean")
+    if _sean_names:
         _post_import.update(_SEAN_MODULES)
     if _post_import:
         if _patcher not in sys.meta_path:
@@ -244,7 +252,8 @@ def uninstall() -> None:
     for module in _patched_parsing:
         importlib.import_module("hairfastgan_b200.parsing_fast").unpatch_parsing_module(module)
     _patched_parsing.clear()
-    for module, ref in _sean_saved.items():
-        module.decode_sean = ref
+    for (module, name), ref in _sean_saved.items():
+        setattr(module, name, ref)
     _sean_saved.clear()
+    _sean_names.clear()
     _post_import.clear()

@@ -70,14 +70,20 @@ def to_nchw32(x16: torch.Tensor, dtype: Optional[int] = None):
 
 
 class PackedConv2d:
-    """One nn.Conv2d repacked as a K-major 16-bit GEMM operand (once per weight version)."""
+    """One nn.Conv2d repacked as a K-major 16-bit GEMM operand (once per weight version).
+    ``prepadded``: the input already carries the 1-pixel border (3x3, stride 1; output (H-2) x (W-2)).
+    ``transposed``: ``weight`` [cin, cout, 3, 3] of nn.ConvTranspose2d(3, stride 2, padding 1, output_padding 1)."""
 
     def __init__(self, weight: torch.Tensor, out_scale=None, stride: int = 1, groups: int = 1,
-                 cin_pad: Optional[int] = None, dtype: Optional[int] = None):
+                 cin_pad: Optional[int] = None, dtype: Optional[int] = None, prepadded: bool = False,
+                 transposed: bool = False):
         dt = default_dtype() if dtype is None else dtype
         cout, cin_g, k, _ = weight.shape
+        if transposed:
+            cin_g, cout = cout, cin_g
         cin = cin_g * groups
-        self.desc = _lib.hf_conv2d_desc(cin, cout, cin if cin_pad is None else cin_pad, k, stride, groups, dt)
+        self.desc = _lib.hf_conv2d_desc(cin, cout, cin if cin_pad is None else cin_pad, k, stride, groups, dt,
+                                        int(prepadded), int(transposed))
         lib = _lib.lib()
         nbytes = lib.hf_conv2d_packed_bytes(C.byref(self.desc))
         if nbytes == 0:
@@ -88,12 +94,18 @@ class PackedConv2d:
         _lib.check(lib.hf_conv2d_pack(C.byref(self.desc), w.data_ptr(), _p(sc), self.blob.data_ptr(), _lib.stream_ptr()),
                    "hf_conv2d_pack")
         self.cout, self.k, self.stride, self.dtype = cout, k, stride, dt
+        self.prepadded, self.transposed = prepadded, transposed
 
     def __call__(self, x16: torch.Tensor, shift=None, act: int = 0, slope=None, slope0: float = 0.0, residual16=None,
                  want_y16: bool = True, y16b_affine=None, want_y32: bool = False, act_after_residual: bool = False):
         """Returns (y16 | None, y16b | None, y32 | None)."""
         b, h, w, _ = x16.shape
-        ho, wo = ((h + 1) // 2, (w + 1) // 2) if self.stride == 2 else (h, w)
+        if self.transposed:
+            ho, wo = 2 * h, 2 * w
+        elif self.prepadded:
+            ho, wo = h - 2, w - 2
+        else:
+            ho, wo = ((h + 1) // 2, (w + 1) // 2) if self.stride == 2 else (h, w)
         dev = x16.device
         io = _lib.hf_conv2d_io()
         io.batch, io.height, io.width, io.x16 = b, h, w, x16.data_ptr()
@@ -128,6 +140,28 @@ def channel_mean(x16: torch.Tensor, dtype: Optional[int] = None):
     _lib.check(_lib.lib().hf_channel_mean_nhwc16(x16.data_ptr(), m.data_ptr(), ws.data_ptr(), b, h * w, c, dt,
                                                  _lib.stream_ptr()), "hf_channel_mean_nhwc16")
     return m
+
+
+def instance_norm_lrelu(x16: torch.Tensor, slope: float = 0.2, dtype: Optional[int] = None):
+    """InstanceNorm2d(affine=False) + LeakyReLU(slope) of [B,H,W,C] 16-bit NHWC -> same shape."""
+    dt = default_dtype() if dtype is None else dtype
+    b, h, w, c = x16.shape
+    y = torch.empty_like(x16)
+    ws = torch.empty(_lib.lib().hf_instance_norm_workspace_bytes(b, h * w, c), device=x16.device, dtype=torch.uint8)
+    _lib.check(_lib.lib().hf_instance_norm_lrelu_nhwc16(x16.data_ptr(), y.data_ptr(), ws.data_ptr(), b, h * w, c,
+                                                        float(slope), dt, _lib.stream_ptr()),
+               "hf_instance_norm_lrelu_nhwc16")
+    return y
+
+
+def reflect_pad1(x16: torch.Tensor, dtype: Optional[int] = None):
+    """ReflectionPad2d(1) of [B,H,W,C] 16-bit NHWC -> [B,H+2,W+2,C]."""
+    dt = default_dtype() if dtype is None else dtype
+    b, h, w, c = x16.shape
+    y = torch.empty(b, h + 2, w + 2, c, device=x16.device, dtype=x16.dtype)
+    _lib.check(_lib.lib().hf_reflect_pad1_nhwc16(x16.data_ptr(), y.data_ptr(), b, h, w, c, dt, _lib.stream_ptr()),
+               "hf_reflect_pad1_nhwc16")
+    return y
 
 
 def se_gate(x16: torch.Tensor, fc1_weight: torch.Tensor, fc2_weight: torch.Tensor, dtype: Optional[int] = None):

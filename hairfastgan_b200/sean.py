@@ -1,4 +1,5 @@
-"""SEAN's ``decode_sean`` (models/sean_codes/models/pix2pix_model.py:309-325) on the sm_90a kernels.
+"""SEAN's ``decode_sean`` (models/sean_codes/models/pix2pix_model.py:309-325) and ``encode_sean`` (:299-306) on the
+sm_90a kernels.
 
 ``decode_sean(sean_model, image_code, target_mask)`` has the reference's signature and result ([3,256,256] fp32 on the
 device of ``target_mask``).  It runs the UI_mode forward of ``sean_model.netG`` (``SPADEGenerator``,
@@ -18,6 +19,13 @@ No host synchronisation except one read of the out-of-range label count.  The 18
 call is the reference's; ``noise=`` injects explicit draws instead.  The Zencoder pass UI_mode runs on an empty
 placeholder batch has no effect and is skipped.  Activations are 16-bit NHWC in the encoder family's type
 (``nn16.default_dtype``, fp16 unless HAIRFAST_ENC_DTYPE / HAIRFAST_DTYPE say bf16).
+
+``encode_sean(sean_model, images, labels)`` runs ``sean_model.netG.Zencoder`` (architecture.py:154-207) for a batch:
+reflection pads (``hf_reflect_pad1_nhwc16``) in front of the prepadded 3x3 convolutions, the two stride-2
+convolutions, the ConvTranspose2d in its four-parity form, all on the wgmma convolution; InstanceNorm + LeakyReLU
+(``hf_instance_norm_lrelu_nhwc16``); tanh and the per-class means over the nearest 128^2 label map
+(``hf_sean_class_means``).  The biases of the four convolutions in front of an InstanceNorm cancel in it and are not
+applied.  One host synchronisation: the read of the out-of-range label count.
 """
 from __future__ import annotations
 
@@ -44,6 +52,15 @@ SUPPORTED_OPT = {"ngf": 64, "label_nc": 19, "semantic_nc": 19, "crop_size": 256,
                  "contain_dontcare_label": False}
 
 _mean_codes_cache = {}
+MAP_SIZE = sum(r * r for r in LEVELS)                        # int8 entries hf_sean_labels writes per sample
+CODE_RES = 128                                               # the Zencoder's code map (architecture.py:178-181)
+MAP_OFFSET_128 = sum(r * r for r in LEVELS[:LEVELS.index(CODE_RES)])
+# Zencoder(3, 512, ngf 32, n_downsampling 2) (architecture.py:154-175, pix2pix SEAN_OPT): state_dict key -> shape.
+# model.10 is the ConvTranspose2d(128, 256) (weight [cin, cout, 3, 3]); the InstanceNorms have no parameters.
+ZENCODER_SHAPES = {"model.1.weight": (32, 3, 3, 3), "model.1.bias": (32,), "model.4.weight": (64, 32, 3, 3),
+                   "model.4.bias": (64,), "model.7.weight": (128, 64, 3, 3), "model.7.bias": (128,),
+                   "model.10.weight": (128, 256, 3, 3), "model.10.bias": (256,), "model.14.weight": (512, 256, 3, 3),
+                   "model.14.bias": (512,)}
 
 
 def check_opt(opt) -> None:
@@ -166,6 +183,40 @@ def noise_resolutions() -> List[int]:
     return [res for _, fin, fout, res, _ in BLOCKS for _ in range(3 if fin != fout else 2)]
 
 
+class PackedZencoder:
+    """Zencoder parameters in the kernels' layouts (once per parameter version)."""
+
+    def __init__(self, zenc, dtype: Optional[int] = None):
+        sd = zenc.state_dict()
+        got = {k: tuple(v.shape) for k, v in sd.items()}
+        if got != ZENCODER_SHAPES:
+            raise NotImplementedError(f"encode_sean: only HairFast's Zencoder(3, 512, ngf 32, n_downsampling 2) is "
+                                      f"supported; its parameters are {ZENCODER_SHAPES}, got {got}")
+        self.dtype = nn16.default_dtype() if dtype is None else dtype
+        self.device = sd["model.1.weight"].device
+        if self.device.type != "cuda":
+            raise RuntimeError("encode_sean: the SEAN model must be on a CUDA device (no CPU fallback)")
+        _lib.use_device(self.device.index)
+        w = lambda i: sd[f"model.{i}.weight"].float()
+        dt = self.dtype
+        # the biases of model.1 / 4 / 7 / 10 are constant per channel and cancel in the InstanceNorm that follows
+        self.conv1 = nn16.PackedConv2d(w(1), cin_pad=32, prepadded=True, dtype=dt)
+        self.conv4 = nn16.PackedConv2d(w(4), stride=2, dtype=dt)
+        self.conv7 = nn16.PackedConv2d(w(7), stride=2, dtype=dt)
+        self.conv10 = nn16.PackedConv2d(w(10), stride=2, transposed=True, dtype=dt)
+        self.conv14 = nn16.PackedConv2d(w(14), prepadded=True, dtype=dt)
+        self.bias14 = sd["model.14.bias"].float().contiguous()
+
+
+def _pack_zencoder(zenc) -> PackedZencoder:
+    key = (_params_key(zenc), nn16.default_dtype())
+    pk = zenc.__dict__.get("_hf_zencoder_pack")
+    if pk is None or pk[0] != key:
+        pk = (key, PackedZencoder(zenc))
+        zenc.__dict__["_hf_zencoder_pack"] = pk
+    return pk[1]
+
+
 # ------------------------------------------------------------------------------------------------ kernel wrappers
 def label_maps(target_mask: torch.Tensor) -> List[torch.Tensor]:
     """[1,1,256,256] labels -> int8 maps at 8..256.  Raises ValueError for labels outside 0..18."""
@@ -264,6 +315,66 @@ def run_block(pk: PackedSEAN, blk: _PackedBlock, x, L, noise_iter, table_iter):
     return x
 
 
+# ------------------------------------------------------------------------------------------------ encode
+def batch_label_maps(labels: torch.Tensor):
+    """[B,1,256,256] labels -> (int8 maps [B, MAP_SIZE] (hf_sean_labels per sample), out-of-range counts [B] int32)."""
+    b = labels.shape[0]
+    lab = labels.reshape(b, SIZE, SIZE).long().contiguous()         # preprocess_input's .long() (pix2pix_model.py:126)
+    maps = torch.empty(b, MAP_SIZE, dtype=torch.int8, device=lab.device)
+    bad = torch.empty(b, dtype=torch.int32, device=lab.device)
+    for i in range(b):
+        _lib.check(_lib.lib().hf_sean_labels(lab[i].data_ptr(), maps[i].data_ptr(), bad[i:].data_ptr(), SIZE,
+                                             _lib.stream_ptr()), "hf_sean_labels")
+    return maps, bad
+
+
+def class_means(y32: torch.Tensor, maps: torch.Tensor) -> torch.Tensor:
+    """tanh + per-class means of the last conv's [B,512,128,128] fp32 output over the 128^2 label maps: [B,19,512]."""
+    b, c, h, w = y32.shape
+    codes = torch.empty(b, N_CLASSES, c, device=y32.device, dtype=torch.float32)
+    _lib.check(_lib.lib().hf_sean_class_means(y32.data_ptr(), maps[:, MAP_OFFSET_128:].data_ptr(), MAP_SIZE,
+                                              codes.data_ptr(), b, c, h * w, _lib.stream_ptr()), "hf_sean_class_means")
+    return codes
+
+
+@torch.no_grad()
+def run_zencoder(pk: PackedZencoder, images: torch.Tensor, maps: torch.Tensor, taps: Optional[dict] = None):
+    """Zencoder.forward (architecture.py:177-207) on [B,3,256,256] images and hf_sean_labels maps -> [B,19,512].
+    ``taps`` receives the four InstanceNorm + LeakyReLU outputs (16-bit NHWC) and the pre-tanh conv (fp32 NCHW)."""
+    dt = pk.dtype
+    x = nn16.reflect_pad1(nn16.to_nhwc16(images, c_pad=32, dtype=dt), dt)             # ReflectionPad2d(1) (:159)
+    for i, conv in enumerate((pk.conv1, pk.conv4, pk.conv7, pk.conv10)):
+        x, _, _ = conv(x)
+        x = nn16.instance_norm_lrelu(x, 0.2, dt)
+        if taps is not None:
+            taps[f"in{i + 1}"] = x
+    _, _, y32 = pk.conv14(nn16.reflect_pad1(x, dt), shift=pk.bias14, want_y16=False, want_y32=True)
+    if taps is not None:
+        taps["pre_tanh"] = y32
+    return class_means(y32, maps)
+
+
+def encode_sean(sean_model, images, labels):
+    """Drop-in for models.sean_codes.models.pix2pix_model.encode_sean: [B,19,512] fp32 style codes on images'
+    device.  Raises ValueError for labels outside 0..18."""
+    zenc = sean_model.netG.Zencoder
+    if not images.is_cuda or not labels.is_cuda:
+        raise RuntimeError("encode_sean: images and labels must be CUDA tensors (no CPU fallback)")
+    if (images.dim() != 4 or labels.dim() != 4 or images.shape[0] < 1 or tuple(images.shape[1:]) != (3, SIZE, SIZE)
+            or tuple(labels.shape) != (images.shape[0], 1, SIZE, SIZE)):
+        raise NotImplementedError(f"encode_sean: images must be [B,3,{SIZE},{SIZE}] and labels [B,1,{SIZE},{SIZE}], "
+                                  f"got {list(images.shape)} and {list(labels.shape)}")
+    pk = _pack_zencoder(zenc)
+    _lib.use_device(images.device.index)
+    maps, bad = batch_label_maps(labels)
+    codes = run_zencoder(pk, images, maps)
+    n_bad = int(bad.sum().item())
+    if n_bad:
+        raise ValueError(f"encode_sean: {n_bad} labels are outside 0..{N_CLASSES - 1}")
+    return codes
+
+
+# ------------------------------------------------------------------------------------------------ decode
 def decode_sean(sean_model, image_code, target_mask, noise: Optional[Sequence[torch.Tensor]] = None,
                 mean_codes: Optional[torch.Tensor] = None):
     """Drop-in for models.sean_codes.models.pix2pix_model.decode_sean: [3,256,256] fp32 on target_mask's device.

@@ -205,6 +205,13 @@ typedef struct {
   int stride;      /* 1 or 2 */
   int groups;      /* >= 1; used to run the 18 GradualStyleBlock heads as one grouped conv */
   int dtype;
+  /* 1: the stored input already carries the 1-pixel border (e.g. nn.ReflectionPad2d(1), which the TMA zero fill cannot
+   * produce): no padding is added and the output is (H-2) x (W-2) of the stored H x W.  ksize 3, stride 1. */
+  int prepadded;
+  /* 1: nn.ConvTranspose2d(cin, cout, 3, stride=2, padding=1, output_padding=1): weight [cin, cout, 3, 3], output
+   * 2H x 2W.  Runs as four 3x3 correlations, one per output parity (4x the algorithmic FLOPs); stride must be 2,
+   * groups 1. */
+  int transposed;
 } hf_conv2d_desc;
 
 size_t hf_conv2d_packed_bytes(const hf_conv2d_desc* d);
@@ -243,6 +250,18 @@ int hf_nchw_to_nhwc16(const float* x, const float* scale, const float* shift, vo
 /* x16 [B,H,W,C] 16-bit NHWC -> y [B,C,H,W] fp32 NCHW */
 int hf_nhwc16_to_nchw(const void* x16, float* y, int batch, int channels, int height, int width, int dtype,
                       void* stream);
+/* SEAN's Zencoder (models/sean_codes/models/networks/architecture.py:154-207) around hf_conv2d_forward. */
+/* Scratch (bytes) of hf_instance_norm_lrelu_nhwc16. */
+size_t hf_instance_norm_workspace_bytes(int batch, int hw, int channels);
+/* nn.InstanceNorm2d(affine=False, track_running_stats=False) + nn.LeakyReLU(slope) on x16 [B,HW,C] 16-bit NHWC -> y16
+ * (may alias x16): per-(b, c) mean, then the biased variance of the centred values (two passes, eps 1e-5), fp32
+ * statistics in a fixed summation order (the reduction of hf_channel_mean_nhwc16).  channels % 8 == 0. */
+int hf_instance_norm_lrelu_nhwc16(const void* x16, void* y16, void* workspace, int batch, int hw, int channels,
+                                  float slope, int dtype, void* stream);
+/* nn.ReflectionPad2d(1): x16 [B,H,W,C] -> y16 [B,H+2,W+2,C] 16-bit NHWC.  H, W >= 2, channels % 8 == 0. */
+int hf_reflect_pad1_nhwc16(const void* x16, void* y16, int batch, int height, int width, int channels, int dtype,
+                           void* stream);
+
 /* Scratch (bytes) for the two-stage deterministic channel reduction below. */
 size_t hf_channel_reduce_workspace_bytes(int batch, int hw, int channels);
 /* SEModule.avg_pool (helpers.py:60): mean over H*W -> [B,C] fp32.  channels % 8 == 0. */
@@ -378,6 +397,13 @@ int hf_sean_ace_apply(const void* x16, const float* noise, const float* noise_va
  * [3][3], bias [3] -> y [3,res,res] fp32 NCHW.  channels % 8 == 0, <= 256. */
 int hf_sean_conv_img(const void* x16, const float* weight, const float* bias, float* y, int res, int channels,
                      int dtype, void* stream);
+
+/* Zencoder.forward's tail (architecture.py:177-207) for one batch: codes[b][j][c] = mean over the pixels p with
+ * labels[b * label_stride + p] == j of tanh(y[b][c][p]), exactly 0 where class j has no pixel.  y [B,channels,hw]
+ * fp32 NCHW (the last conv's output, bias included); labels int8 (hf_sean_labels' 128^2 level per sample); codes
+ * [B,19,channels] fp32.  Fixed summation order, no atomics. */
+int hf_sean_class_means(const float* y, const int8_t* labels, long long label_stride, float* codes, int batch,
+                        int channels, int hw, void* stream);
 
 /* Number of kernels the last hf_generator_forward / hf_conv_forward of this thread launched. */
 int hf_last_launch_count(void);

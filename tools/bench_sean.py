@@ -1,6 +1,7 @@
-"""Time SEAN's decode_sean: the stock reference against hairfastgan_b200.sean, same GPU, same synthetic weights, B = 1.
+"""Time SEAN's decode_sean (and, with --encode, encode_sean): the stock reference against hairfastgan_b200.sean, same
+GPU, same synthetic weights; decode B = 1, encode B = 2 (what Alignment.align_images passes, models/Alignment.py:128).
 
-    python tools/bench_sean.py [--reps 20] [--warmup 3] [--swap] [--out result.json]
+    python tools/bench_sean.py [--reps 20] [--warmup 3] [--encode] [--swap] [--out result.json]
 
 * both decodes run on ONE reference ``Pix2PixModel(SEAN_OPT)`` built by the reference's own code from a checkpoint
   holding ``oracle.sean_oracle.synth_sean_params(5)`` (needs the reference built under oracle/_ref, baseline/refenv.py);
@@ -9,7 +10,10 @@
   other (upsample, conv_img);
 * achieved TFLOP/s against the algorithmic FLOPs of the decode, the lookup-replaced convolutions counted at their
   convolution FLOPs (the rule of bench.py's roofline);
-* --swap: full_swap_ms / out_of_scope_ms of baseline/run_swap.py for the overlay and overlay_sean arms;
+* --encode: the same timing of encode_sean, its algorithmic FLOPs (the ConvTranspose2d counted at its algorithmic
+  FLOPs, a quarter of what its four-parity form runs) and the max difference of the codes;
+* --swap: full_swap_ms / out_of_scope_ms of baseline/run_swap.py for the overlay, overlay_sean and overlay_sean_full
+  arms;
 * the card name, power limit and SM clock are read in the same run (nvidia-smi queries only).
 """
 from __future__ import annotations
@@ -43,6 +47,14 @@ def decode_flops() -> float:
         if fin != fout:
             f += 2 * fin * fout * hw                                # conv_s
     return f + 2 * 64 * 3 * 9 * 256 * 256                          # conv_img
+
+
+def encode_flops(batch: int = 2) -> float:
+    """Algorithmic FLOPs of one encode_sean call (2 per MAC): the five Zencoder convolutions (architecture.py:154-175)."""
+    f = 2 * 3 * 32 * 9 * 256 ** 2 + 2 * 32 * 64 * 9 * 128 ** 2 + 2 * 64 * 128 * 9 * 64 ** 2
+    f += 2 * 128 * 256 * 9 * 64 ** 2                               # ConvTranspose2d: 9 taps per input pixel
+    f += 2 * 256 * 512 * 9 * 128 ** 2
+    return batch * f
 
 
 def gpu_info():
@@ -100,7 +112,7 @@ def stage_split(fn):
 def swap_arms(work):
     res = {}
     env = {k: v for k, v in os.environ.items() if k not in ("HAIRFAST_DTYPE", "HAIRFAST_ENC_DTYPE")}
-    for mode in ("overlay", "overlay_sean"):
+    for mode in ("overlay", "overlay_sean", "overlay_sean_full"):
         out = os.path.join(tempfile.mkdtemp(), mode + ".pt")
         cmd = [sys.executable, os.path.join(ROOT, "baseline", "run_swap.py"), "--mode", mode, "--work", work,
                "--out", out, "--reps", "3", "--warmup", "1"]
@@ -118,10 +130,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--encode", action="store_true", help="also time encode_sean")
     ap.add_argument("--swap", action="store_true")
     ap.add_argument("--work", default="/tmp/hairfast_work")
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     a = ap.parse_args()
+    out_path = os.path.abspath(a.out) if a.out else None     # refenv.activate changes the working directory
 
     from baseline import refenv
     if not refenv.available():
@@ -165,11 +179,27 @@ def main():
            "ours_ms_all": [round(x, 3) for x in ours_all], "ours_stage_kernel_ms": stages,
            "algorithmic_gflop": round(flops / 1e9, 1), "ours_tflops": round(flops / ours_ms / 1e9, 1),
            "stock_tflops": round(flops / stock_ms / 1e9, 1), "max_abs_vs_stock": diff}
+    if a.encode:
+        images = (torch.rand(2, 3, 256, 256, generator=g) * 2 - 1).to(dev)
+        enc_labels = torch.randint(0, 19, (2, 1, 16, 16), generator=g).repeat_interleave(16, 2).repeat_interleave(16, 3)
+        enc_labels = enc_labels.float().to(dev)
+        with torch.inference_mode():
+            ref_codes = P.encode_sean(model, images, enc_labels)
+            our_codes = S.encode_sean(model, images, enc_labels)
+            stock_e, stock_e_all = time_calls(lambda: P.encode_sean(model, images, enc_labels), a.reps, a.warmup, flush)
+            ours_e, ours_e_all = time_calls(lambda: S.encode_sean(model, images, enc_labels), a.reps, a.warmup, flush)
+        ef = encode_flops(2)
+        res["encode"] = {"batch": 2, "stock_encode_ms": round(stock_e, 3), "ours_encode_ms": round(ours_e, 3),
+                         "speedup": round(stock_e / ours_e, 2), "stock_ms_all": [round(x, 3) for x in stock_e_all],
+                         "ours_ms_all": [round(x, 3) for x in ours_e_all], "algorithmic_gflop": round(ef / 1e9, 2),
+                         "ours_tflops": round(ef / ours_e / 1e9, 1), "stock_tflops": round(ef / stock_e / 1e9, 1),
+                         "codes_max_abs_vs_stock": float((our_codes - ref_codes).abs().max()),
+                         "codes_max_abs_ref": float(ref_codes.abs().max())}
     if a.swap:
         res["swap"] = swap_arms(os.path.abspath(a.work))
     print(json.dumps(res))
-    if a.out:
-        with open(a.out, "w") as f:
+    if out_path:
+        with open(out_path, "w") as f:
             json.dump(res, f, indent=1)
 
 
