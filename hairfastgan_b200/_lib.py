@@ -153,6 +153,14 @@ SYMBOLS = {
                                       C.c_void_p]),
     "hf_sean_conv_img": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                    C.c_void_p]),
+    "hf_shape_labels": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "hf_shape_onehot_s2": (C.c_int, [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "hf_shape_gemm": (C.c_int, [C.c_int] + [C.c_void_p] * 6 + [C.c_int] * 5 + [C.c_void_p]),
+    "hf_shape_gemm_workspace_bytes": (C.c_size_t, [C.c_int] * 5),
+    "hf_shape_gemm_plan": (C.c_int, [C.c_int] * 6 + [C.POINTER(C.c_int)]),
+    "hf_shape_layer_norm_lrelu": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p]),
+    "hf_shape_layer_norm_workspace_bytes": (C.c_size_t, [C.c_longlong]),
+    "hf_shape_logits_argmax": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_void_p]),
     "hf_generator_packed_bytes":(C.c_size_t, [C.POINTER(hf_gen_config)]),
     "hf_generator_workspace_bytes": (C.c_size_t, [C.POINTER(hf_gen_config), C.c_int]),
     "hf_generator_pack": (C.c_int, [C.POINTER(hf_gen_config), C.POINTER(hf_gen_weights), C.c_void_p, C.c_void_p]),

@@ -38,6 +38,9 @@ After ``install()`` the import statements of the reference resolve to this packa
                                                                                     -> ``hairfastgan_b200.sean``
 * opt-in, ``install(sean_encode=True)``: ``encode_sean`` (pix2pix_model.py:299-306) is rebound in the same two modules
                                                                                     -> ``hairfastgan_b200.sean``
+* opt-in, ``install(shape_adaptor=True)``: CtrlHair's ``get_hair_face_code`` and ``get_new_shape``
+  (models/CtrlHair/shape_branch/solver.py:248-262) are rebound inside that module and ``models.Alignment`` (which
+  imports both names, Alignment.py:7)                                               -> ``hairfastgan_b200.shape_adaptor``
 
 Nothing in the reference tree is edited and its JIT build of the two 2019 CUDA extensions
 (op/fused_act.py:10-16, op/upfirdn2d.py:10-16) never runs.
@@ -94,8 +97,14 @@ _FSE_TRAINER = "trainer"
 # face parsing: FaceParsing_tensor.parsing_img (my_parsing_util.py:70-89) -> label-only path of hairfastgan_b200/parsing_fast.py
 _PARSING_UTIL = "models.CtrlHair.external_code.face_parsing.my_parsing_util"
 _patched_parsing = []
-# SEAN (opt-in): the function names rebound in these modules, and (module, name) -> the reference function it held
+# SEAN and the shape adaptor (opt-in): function name -> (our module, the modules that hold the name; the first defines
+# it), the names chosen by install(), and (module, name) -> the reference function it held
 _SEAN_MODULES = ("models.sean_codes.models.pix2pix_model", "models.Alignment")
+_SHAPE_MODULES = ("models.CtrlHair.shape_branch.solver", "models.Alignment")
+_FUNCTIONS = {"decode_sean": ("hairfastgan_b200.sean", _SEAN_MODULES),
+              "encode_sean": ("hairfastgan_b200.sean", _SEAN_MODULES),
+              "get_hair_face_code": ("hairfastgan_b200.shape_adaptor", _SHAPE_MODULES),
+              "get_new_shape": ("hairfastgan_b200.shape_adaptor", _SHAPE_MODULES)}
 _sean_names = set()
 _sean_saved = {}
 _post_import = set()          # module names the meta-path hook currently patches
@@ -103,11 +112,12 @@ _patched_trainers = []
 
 
 def _patch_sean(module, name: str) -> None:
-    ours = getattr(importlib.import_module("hairfastgan_b200.sean"), name)
+    ours_module, modules = _FUNCTIONS[name]
+    ours = getattr(importlib.import_module(ours_module), name)
     current = getattr(module, name, None)
     if current is None or current is ours:
-        # models.Alignment imported the name after pix2pix_model was rebound: restore it to the reference's function
-        ref = sys.modules.get(_SEAN_MODULES[0])
+        # models.Alignment imported the name after the defining module was rebound: restore it to the reference's
+        ref = sys.modules.get(modules[0])
         if current is ours and ref is not None and (ref, name) in _sean_saved and (module, name) not in _sean_saved:
             _sean_saved[(module, name)] = _sean_saved[(ref, name)]
         return
@@ -116,9 +126,10 @@ def _patch_sean(module, name: str) -> None:
 
 
 def _patch_postprocess(module) -> None:
-    if module.__name__ in _SEAN_MODULES:
+    if module.__name__ in _SEAN_MODULES + _SHAPE_MODULES:
         for name in sorted(_sean_names):
-            _patch_sean(module, name)
+            if module.__name__ in _FUNCTIONS[name][1]:
+                _patch_sean(module, name)
         return
     if module.__name__ == _PARSING_UTIL:
         fast = importlib.import_module("hairfastgan_b200.parsing_fast")
@@ -192,12 +203,13 @@ def _register(ref_name: str, ours: str) -> None:
 
 def install(generator: bool = True, encoders: bool = True, postprocess: bool = True, segmentation: bool = True,
             glue: bool = True, skip_fse_reconstruction: bool = False, fuse_face_parsing: bool = True,
-            sean: bool = False, sean_encode: bool = False) -> None:
+            sean: bool = False, sean_encode: bool = False, shape_adaptor: bool = False) -> None:
     """Register the overlay.  ``generator=False`` swaps only the operator package (L1 boundary) and leaves the
     reference's own ``models/stylegan2/model.py`` classes in place on top of our ops; ``encoders=False`` keeps
     the reference's PyTorch encoders; ``postprocess=False`` keeps its PostProcess conv stack; ``segmentation=False``
     its BiSeNet.  ``sean=True`` (off by default) runs SEAN's ``decode_sean`` on our kernels; ``sean_encode=True`` (off
-    by default, independent of ``sean``) runs its ``encode_sean`` (the Zencoder) on them."""
+    by default, independent of ``sean``) runs its ``encode_sean`` (the Zencoder) on them; ``shape_adaptor=True`` (off by
+    default) runs CtrlHair's shape adaptor (``get_hair_face_code`` / ``get_new_shape``) on them."""
     if segmentation:
         for ref_name, ours in _SEGMENTATION.items():
             _register(ref_name, ours)
@@ -227,8 +239,10 @@ def install(generator: bool = True, encoders: bool = True, postprocess: bool = T
         _sean_names.add("decode_sean")
     if sean_encode:
         _sean_names.add("encode_sean")
-    if _sean_names:
-        _post_import.update(_SEAN_MODULES)
+    if shape_adaptor:
+        _sean_names.update(("get_hair_face_code", "get_new_shape"))
+    for name in _sean_names:
+        _post_import.update(_FUNCTIONS[name][1])
     if _post_import:
         if _patcher not in sys.meta_path:
             sys.meta_path.insert(0, _patcher)

@@ -405,6 +405,43 @@ int hf_sean_conv_img(const void* x16, const float* weight, const float* bias, fl
 int hf_sean_class_means(const float* y, const int8_t* labels, long long label_stride, float* codes, int batch,
                         int channels, int hw, void* stream);
 
+/* ---- CtrlHair shape adaptor (models/CtrlHair/shape_branch/model.py:146-199) ---- */
+/* mask_label_to_one_hot's label side (shape_util.py:6-14): mask [n] int64 is rewritten 255 -> 19 in place; labels
+ * [n] int8 gets 0..19 (19 = the all-zero one-hot); *bad = the count of values outside {0..19, 255}. */
+int hf_shape_labels(long long* mask, int8_t* labels, int* bad, int n, void* stream);
+
+/* MaskEncoder layer 0 (ZeroPad 1 + Conv 4x4 stride 2) as a lookup: y16[p][c] = cmap[p][c] + sum over the taps inside
+ * the (2 res)^2 label map of table[tap][label][c].  labels [2res][2res] int8 (hf_shape_labels); table [16][20][channels]
+ * fp32 (tap = ky*4 + kx); cmap [res*res][channels] fp32 (positional channels' conv + bias); y16 [res,res,channels]
+ * 16-bit NHWC.  channels % 8 == 0. */
+int hf_shape_onehot_s2(const int8_t* labels, const float* table, const float* cmap, void* y16, int res, int channels,
+                       int dtype, void* stream);
+
+/* Split-K GEMM with compact 16-bit weights w16 [cout][K] (k = tap*cin + c) and the im2col gathered from x16
+ * [hin,win,cin] 16-bit NHWC.  mode 0: 1x1 / Linear (P = hin*win, K = cin); mode 1: ZeroPad 1 + Conv 4x4 stride 2
+ * (P = hin/2 * win/2, K = 16 cin); mode 2: nearest 2x upsample + Conv 3x3 pad 1 (P = 4 hin win, K = 9 cin).
+ * y[p][co] = bias[co] + sum_k (fp32 partials per split, added in split order) -> y32 fp32 and / or y16 16-bit, both
+ * [P][cout].  cin % 8 == 0; workspace hf_shape_gemm_workspace_bytes. */
+int hf_shape_gemm(int mode, const void* w16, const void* x16, const float* bias, float* y32, void* y16, float* workspace,
+                  int cin, int cout, int hin, int win, int dtype, void* stream);
+size_t hf_shape_gemm_workspace_bytes(int mode, int cin, int cout, int hin, int win);
+/* The plan hf_shape_gemm picks on a device with `sms` SMs (needs no device): out[5] = {pixel tile, K splits, 64-wide
+ * K tiles, cout tiles, pixel tiles}. */
+int hf_shape_gemm_plan(int mode, int cin, int cout, int hin, int win, int sms, int* out);
+
+/* CtrlHair LayerNorm (my_torchlib/module.py:183-205) over the whole [pixels, channels] 16-bit NHWC sample, then
+ * LeakyReLU(slope): (x - mean) / (unbiased std + 1e-5) * gamma[c] + beta[c].  Fixed-order fp32 statistics.
+ * workspace hf_shape_layer_norm_workspace_bytes(pixels * channels). */
+int hf_shape_layer_norm_lrelu(const void* x16, const float* gamma, const float* beta, void* y16, float* workspace,
+                              int pixels, int channels, float slope, int dtype, void* stream);
+size_t hf_shape_layer_norm_workspace_bytes(long long n);
+
+/* Both decoders' out_layer (Conv 3x3 pad 1 over the 32-channel maps hair16 / face16 [res,res,32] 16-bit NHWC) and the
+ * argmax over cat[face[:13], hair, face[13:]]: table [19][9][32] fp32 in that channel order, bias [19];
+ * labels [res*res] int64, ties to the first index. */
+int hf_shape_logits_argmax(const void* hair16, const void* face16, const float* table, const float* bias,
+                           long long* labels, int res, int dtype, void* stream);
+
 /* Number of kernels the last hf_generator_forward / hf_conv_forward of this thread launched. */
 int hf_last_launch_count(void);
 /* Number of kernels every hf_* call of this thread has launched since the library was loaded. */
