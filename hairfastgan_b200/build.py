@@ -11,7 +11,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libhairfast_sm90.so")
-SOURCES = ["hf_api.cu", "hf_ops.cu", "hf_conv_tc.cu", "hf_generator.cu", "hf_enc_ops.cu", "hf_enc_api.cu",
+SOURCES = ["hf_api.cu", "hf_ops.cu", "hf_conv_tc.cu", "hf_generator.cu", "hf_enc_ops.cu",
            "hf_seg_ops.cu", "hf_glue_ops.cu", "hf_sean.cu",
            "hf_shape.cu"]
 HEADERS = ["hf_common.cuh", "hf_kernels.cuh", os.path.join("..", "..", "include", "hairfast_b200.h")]

@@ -1,5 +1,6 @@
-// C-ABI entry points (include/hairfast_b200.h) for the operator- and module-level calls, plus the
-// process-wide plumbing: thread-local error string, device selection, TMA descriptor encoding.
+// C-ABI entry points (include/hairfast_b200.h) of the convolution descriptors (hf_conv_*, hf_conv2d_*) and ToRGB,
+// plus the process-wide plumbing: thread-local error string, device selection, TMA descriptor encoding.  The SIMT
+// entry points live beside their kernels.
 #include <stdarg.h>
 #include <string.h>
 
@@ -100,7 +101,40 @@ static int check_desc(const hf_conv_desc* d) {
   return HF_OK;
 }
 
-static int ensure_device() {
+static int check_conv2d(const hf_conv2d_desc* d) {
+  HF_REQUIRE(d, "conv2d: null descriptor");
+  HF_REQUIRE(d->dtype == HF_BF16 || d->dtype == HF_F16, "conv2d: bad dtype %d", d->dtype);
+  HF_REQUIRE(d->ksize == 1 || d->ksize == 3, "conv2d: kernel size %d unsupported (1 or 3)", d->ksize);
+  HF_REQUIRE(d->stride == 1 || d->stride == 2, "conv2d: stride %d unsupported (1 or 2)", d->stride);
+  HF_REQUIRE(d->groups >= 1 && d->cin > 0 && d->cout > 0 && d->cin % d->groups == 0 && d->cout % d->groups == 0,
+             "conv2d: bad channels / groups (%d -> %d, groups %d)", d->cin, d->cout, d->groups);
+  HF_REQUIRE(d->cin_pad >= d->cin && d->cin_pad % (32 * d->groups) == 0,
+             "conv2d: cin_pad=%d must be >= cin and a multiple of 32 per group", d->cin_pad);
+  HF_REQUIRE(d->groups == 1 || d->cin_pad == d->cin, "conv2d: channel padding is not supported with groups > 1");
+  HF_REQUIRE(d->cout % 32 == 0, "conv2d: cout=%d must be a multiple of 32", d->cout);
+  HF_REQUIRE((d->prepadded == 0 || d->prepadded == 1) && (d->transposed == 0 || d->transposed == 1),
+             "conv2d: prepadded / transposed must be 0 or 1");
+  HF_REQUIRE(!d->prepadded || (d->ksize == 3 && d->stride == 1 && !d->transposed),
+             "conv2d: a prepadded input needs a stride-1 3x3 conv");
+  HF_REQUIRE(!d->transposed || (d->ksize == 3 && d->stride == 2 && d->groups == 1),
+             "conv2d: the transposed form is ConvTranspose2d(3, stride 2, padding 1, output_padding 1), no groups");
+  return HF_OK;
+}
+
+// the shape half of the launch: what conv_plan reads
+static ConvLaunch conv2d_launch_shape(const hf_conv2d_desc* d, int batch, int height, int width) {
+  ConvLaunch cl;
+  memset(&cl, 0, sizeof(cl));
+  cl.B = batch; cl.H = height; cl.W = width;
+  cl.Cin = d->cin_pad; cl.Cout = d->cout;
+  cl.taps = d->ksize * d->ksize; cl.dtype = d->dtype;
+  cl.stride = d->transposed ? 1 : d->stride; cl.groups = d->groups;   // transposed: the four-parity 3x3 form
+  cl.up = d->transposed; cl.prepadded = d->prepadded;
+  cl.epi = 1;
+  return cl;
+}
+
+int ensure_device_current() {
   if (g_device >= 0) {
     int cur = -1;
     cudaGetDevice(&cur);
@@ -108,7 +142,6 @@ static int ensure_device() {
   }
   return HF_OK;
 }
-int ensure_device_current() { return ensure_device(); }
 
 }  // namespace hf
 
@@ -139,26 +172,8 @@ int hf_set_device(int device) {
 }
 
 int hf_sm_count(void) {
-  if (ensure_device()) return -1;
+  if (ensure_device_current()) return -1;
   return num_sms();
-}
-
-int hf_upfirdn2d_f32(const float* x, float* y, const float* kernel, int planes, int in_h, int in_w, int kernel_h,
-                     int kernel_w, int up_x, int up_y, int down_x, int down_y, int pad_x0, int pad_x1, int pad_y0,
-                     int pad_y1, void* stream) {
-  int rc = ensure_device();
-  if (rc) return rc;
-  reset_launch_count();
-  return launch_upfirdn2d(x, y, kernel, planes, in_h, in_w, kernel_h, kernel_w, up_x, up_y, down_x, down_y, pad_x0,
-                          pad_x1, pad_y0, pad_y1, (cudaStream_t)stream);
-}
-
-int hf_bias_act_f32(const float* x, const float* bias, float* y, int64_t n, int size_b, int64_t step_b, int act,
-                    float alpha, float scale, void* stream) {
-  int rc = ensure_device();
-  if (rc) return rc;
-  reset_launch_count();
-  return launch_bias_act(x, bias, y, n, size_b, step_b, act, alpha, scale, (cudaStream_t)stream);
 }
 
 size_t hf_conv_packed_bytes(const hf_conv_desc* d) {
@@ -169,7 +184,7 @@ size_t hf_conv_packed_bytes(const hf_conv_desc* d) {
 int hf_conv_pack(const hf_conv_desc* d, const float* weight, const float* blur_kernel, void* packed, void* stream) {
   int rc = check_desc(d);
   if (rc) return rc;
-  if ((rc = ensure_device())) return rc;
+  if ((rc = ensure_device_current())) return rc;
   HF_REQUIRE(weight && packed, "hf_conv_pack: null pointer");
   HF_REQUIRE(((uintptr_t)packed & 255) == 0, "hf_conv_pack: packed buffer must be 256-byte aligned");
   float* wsq = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(packed) + conv_wpk_bytes(d));
@@ -214,7 +229,7 @@ static int conv_forward_impl(const hf_conv_desc* d, const void* packed, const hf
                              int time_iters, float* avg_ms) {
   int rc = check_desc(d);
   if (rc) return rc;
-  if ((rc = ensure_device())) return rc;
+  if ((rc = ensure_device_current())) return rc;
   reset_launch_count();
   HF_REQUIRE(packed && io && io->x && io->style && io->mod_weight && io->mod_bias && io->y && io->workspace,
              "hf_conv_forward: null pointer");
@@ -269,11 +284,59 @@ static int conv_forward_impl(const hf_conv_desc* d, const void* packed, const hf
   return HF_OK;
 }
 
+size_t hf_conv2d_packed_bytes(const hf_conv2d_desc* d) {
+  if (check_conv2d(d)) return 0;
+  return align256((size_t)(d->transposed ? 4 : 1) * d->cout * d->ksize * d->ksize * (d->cin_pad / d->groups) * 2);
+}
+
+int hf_conv2d_pack(const hf_conv2d_desc* d, const float* weight, const float* out_scale, void* packed, void* stream) {
+  int rc = check_conv2d(d);
+  if (rc) return rc;
+  if ((rc = ensure_device_current())) return rc;
+  HF_REQUIRE(weight && packed && ((uintptr_t)packed & 255) == 0, "hf_conv2d_pack: null / unaligned pointer");
+  if (d->transposed)
+    return launch_pack_conv2d_transposed(weight, out_scale, packed, d->cout, d->cin, d->cin_pad, d->dtype,
+                                         (cudaStream_t)stream);
+  return launch_pack_conv2d(weight, out_scale, packed, d->cout, d->cin / d->groups, d->cin_pad / d->groups, d->ksize,
+                            d->dtype, (cudaStream_t)stream);
+}
+
+int hf_conv2d_forward(const hf_conv2d_desc* d, const void* packed, const hf_conv2d_io* io, void* stream) {
+  int rc = check_conv2d(d);
+  if (rc) return rc;
+  if ((rc = ensure_device_current())) return rc;
+  reset_launch_count();
+  HF_REQUIRE(packed && io && io->x16, "hf_conv2d_forward: null pointer");
+  HF_REQUIRE(io->y16 || io->y16b || io->y32_nchw, "hf_conv2d_forward: no output requested");
+  HF_REQUIRE(io->batch > 0 && io->height > 0 && io->width > 0, "hf_conv2d_forward: bad shape");
+  HF_REQUIRE(io->act != 1 || io->slope, "hf_conv2d_forward: PReLU needs a slope vector");
+  ConvLaunch cl = conv2d_launch_shape(d, io->batch, io->height, io->width);
+  cl.xhat_in = io->x16; cl.wpk = packed;
+  cl.enc_shift = io->shift; cl.enc_act = io->act; cl.enc_slope = io->act == 1 ? io->slope : nullptr;
+  cl.enc_slope0 = io->slope0;
+  cl.enc_residual = io->residual16;
+  cl.enc_post = io->act_after_residual ? 1 : 0;
+  cl.xhat_out = io->y16;
+  cl.enc_s2 = io->y16b_scale; cl.enc_b2 = io->y16b_shift; cl.enc_y16b = io->y16b;
+  cl.out_nchw = io->y32_nchw;
+  return launch_conv(cl, (cudaStream_t)stream, nullptr);
+}
+
+int hf_conv2d_plan_query(const hf_conv2d_desc* d, int batch, int height, int width, int* out) {
+  int rc = check_conv2d(d);
+  if (rc) return rc;
+  HF_REQUIRE(out, "hf_conv2d_plan_query: null output");
+  ConvPlan pl;
+  if ((rc = conv_plan(conv2d_launch_shape(d, batch, height, width), &pl))) return rc;
+  conv_plan_export(pl, out);
+  return HF_OK;
+}
+
 int hf_torgb_forward(const float* x, const float* style, int64_t style_stride, int style_dim,
                      const float* conv_weight, const float* mod_weight, const float* mod_bias, const float* bias,
                      const float* up_kernel, const float* skip, float* y, int batch, int cin, int height, int width,
                      void* workspace, void* stream) {
-  int rc = ensure_device();
+  int rc = ensure_device_current();
   if (rc) return rc;
   reset_launch_count();
   HF_REQUIRE(x && style && conv_weight && mod_weight && mod_bias && y && workspace, "hf_torgb_forward: null pointer");

@@ -8,6 +8,9 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <algorithm>
+#include <type_traits>
+
 #include "../../include/hairfast_b200.h"
 
 namespace hf {
@@ -45,6 +48,20 @@ int encode_tmap(CUtensorMap* map, int dtype, int rank, void* gaddr, const uint64
     }                                                                                      \
   } while (0)
 
+inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
+// grid of a 256-thread grid-stride loop over n items: at most 16 CTAs per SM
+inline int grid_for(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, (int64_t)num_sms() * 16); }
+
+// Calls body(std::integral_constant<int, DT>{}) for dtype HF_BF16 or HF_F16, so that the body instantiates its
+// kernels with a compile-time DT; any other dtype is rejected with "<what>: bad dtype".
+template <class Body>
+int with_dtype(int dtype, const char* what, Body&& body) {
+  if (dtype == HF_BF16) return body(std::integral_constant<int, HF_BF16>{});
+  if (dtype == HF_F16) return body(std::integral_constant<int, HF_F16>{});
+  set_error("%s: bad dtype %d", what, dtype);
+  return HF_ERR_INVALID;
+}
+
 // ----------------------------------------------------------------------------------------
 // 16-bit storage type helpers.  dtype: HF_BF16 (default) or HF_F16.
 // ----------------------------------------------------------------------------------------
@@ -76,6 +93,33 @@ template <> struct Half2T<HF_F16> {
     return __half2float(h);
   }
 };
+
+// eight 16-bit values in one 16-byte word <-> floats
+template <int DT>
+__device__ __forceinline__ void unpack8(const uint4& v, float* f) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    f[2 * k] = Half2T<DT>::to_float((uint16_t)(w[k] & 0xFFFF));
+    f[2 * k + 1] = Half2T<DT>::to_float((uint16_t)(w[k] >> 16));
+  }
+}
+template <int DT>
+__device__ __forceinline__ uint4 pack8(const float* v) {
+  uint4 o;
+  o.x = Half2T<DT>::pack(v[0], v[1]); o.y = Half2T<DT>::pack(v[2], v[3]);
+  o.z = Half2T<DT>::pack(v[4], v[5]); o.w = Half2T<DT>::pack(v[6], v[7]);
+  return o;
+}
+// p 16-byte aligned
+template <int DT>
+__device__ __forceinline__ void ld8(const uint16_t* p, float* f) {
+  unpack8<DT>(__ldg(reinterpret_cast<const uint4*>(p)), f);
+}
+template <int DT>
+__device__ __forceinline__ void st8(uint16_t* p, const float* v) {
+  *reinterpret_cast<uint4*>(p) = pack8<DT>(v);
+}
 
 // ----------------------------------------------------------------------------------------
 // PTX wrappers
@@ -151,7 +195,19 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       "r"(c2), "r"(c3)
       : "memory");
 }
-
+// Warp-level D[16 x 8] += A[16 x 16] * B[16 x 8] (mma.sync m16n8k16, fp32 accumulators): a the four A registers,
+// b0 / b1 the two B registers of this lane's fragment.
+template <int DT>
+__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  if (DT == HF_BF16)
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+  else
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
 
 // --- wgmma (Hopper warpgroup MMA, accumulators in registers) ---------------------------------
 // Shared-memory matrix descriptor (PTX "matrix descriptor format" for wgmma):

@@ -7,20 +7,8 @@
 
 namespace hf {
 
-static inline int cdiv_i(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
-
 template <int DT>
 __device__ __forceinline__ float ld16(const uint16_t* p) { return Half2T<DT>::to_float(*p); }
-
-template <int DT>
-__device__ __forceinline__ void unpack8(const uint4& v, float* f) {
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    f[2 * k] = Half2T<DT>::to_float((uint16_t)(w[k] & 0xFFFF));
-    f[2 * k + 1] = Half2T<DT>::to_float((uint16_t)(w[k] >> 16));
-  }
-}
 
 // wpk[o][tap*cin_pad + c] = w[o, c, tap] * out_scale[o]   (c >= cin -> 0: channel padding of the input)
 template <int DT>
@@ -70,14 +58,13 @@ int launch_pack_conv2d_transposed(const float* w, const float* out_scale, void* 
   HF_REQUIRE(w && wpk, "pack_conv2d_transposed: null pointer");
   HF_REQUIRE(cout % 32 == 0 && cin_pad >= cin && cin_pad % 32 == 0, "pack_conv2d_transposed: bad channels %d -> %d",
              cin, cout);
-  const int grid = cdiv_i((int64_t)4 * cout * cin_pad, 256);
-  if (dtype == HF_BF16)
-    pack_conv2d_transposed_kernel<HF_BF16><<<grid, 256, 0, st>>>(w, out_scale, (uint16_t*)wpk, cout, cin, cin_pad);
-  else
-    pack_conv2d_transposed_kernel<HF_F16><<<grid, 256, 0, st>>>(w, out_scale, (uint16_t*)wpk, cout, cin, cin_pad);
-  HF_LAUNCH_OK("pack_conv2d_transposed");
-  count_launch();
-  return HF_OK;
+  const int grid = cdiv((int64_t)4 * cout * cin_pad, 256);
+  return with_dtype(dtype, "pack_conv2d_transposed", [&](auto dt) -> int {
+    pack_conv2d_transposed_kernel<dt><<<grid, 256, 0, st>>>(w, out_scale, (uint16_t*)wpk, cout, cin, cin_pad);
+    HF_LAUNCH_OK("pack_conv2d_transposed");
+    count_launch();
+    return HF_OK;
+  });
 }
 
 int launch_pack_conv2d(const float* w, const float* out_scale, void* wpk, int cout, int cin_g, int cin_pad, int ksize,
@@ -85,14 +72,13 @@ int launch_pack_conv2d(const float* w, const float* out_scale, void* wpk, int co
   HF_REQUIRE(w && wpk, "pack_conv2d: null pointer");
   HF_REQUIRE(cin_pad >= cin_g && cin_pad % 32 == 0, "pack_conv2d: cin_pad=%d must be >= cin and a multiple of 32", cin_pad);
   const int taps = ksize * ksize;
-  const int grid = cdiv_i((int64_t)cout * cin_pad, 256);
-  if (dtype == HF_BF16)
-    pack_conv2d_kernel<HF_BF16><<<grid, 256, 0, st>>>(w, out_scale, (uint16_t*)wpk, cout, cin_g, cin_pad, taps);
-  else
-    pack_conv2d_kernel<HF_F16><<<grid, 256, 0, st>>>(w, out_scale, (uint16_t*)wpk, cout, cin_g, cin_pad, taps);
-  HF_LAUNCH_OK("pack_conv2d");
-  count_launch();
-  return HF_OK;
+  const int grid = cdiv((int64_t)cout * cin_pad, 256);
+  return with_dtype(dtype, "pack_conv2d", [&](auto dt) -> int {
+    pack_conv2d_kernel<dt><<<grid, 256, 0, st>>>(w, out_scale, (uint16_t*)wpk, cout, cin_g, cin_pad, taps);
+    HF_LAUNCH_OK("pack_conv2d");
+    count_launch();
+    return HF_OK;
+  });
 }
 
 // x [B,C,HW] fp32 -> y16 [B,HW,Cpad]; y = x*scale[c] + shift[c]; channels >= C are zero
@@ -124,20 +110,6 @@ __global__ void __launch_bounds__(256) nchw_to_nhwc16_kernel(const float* __rest
   }
 }
 
-int launch_nchw_to_nhwc16(const float* x, const float* scale, const float* shift, void* y16, int B, int C, int Cpad,
-                          int HW, int dtype, cudaStream_t st) {
-  HF_REQUIRE(x && y16, "nchw_to_nhwc16: null pointer");
-  HF_REQUIRE(Cpad >= C && Cpad % 2 == 0, "nchw_to_nhwc16: bad channel padding %d for %d", Cpad, C);
-  dim3 grid(cdiv_i(HW, 32), cdiv_i(Cpad, 64), B);
-  if (dtype == HF_BF16)
-    nchw_to_nhwc16_kernel<HF_BF16><<<grid, 256, 0, st>>>(x, scale, shift, (uint16_t*)y16, C, Cpad, HW);
-  else
-    nchw_to_nhwc16_kernel<HF_F16><<<grid, 256, 0, st>>>(x, scale, shift, (uint16_t*)y16, C, Cpad, HW);
-  HF_LAUNCH_OK("nchw_to_nhwc16");
-  count_launch();
-  return HF_OK;
-}
-
 // x16 [B,HW,C] -> y fp32 [B,C,HW]
 template <int DT>
 __global__ void __launch_bounds__(256) nhwc16_to_nchw_kernel(const uint16_t* __restrict__ x, float* __restrict__ y,
@@ -156,18 +128,6 @@ __global__ void __launch_bounds__(256) nhwc16_to_nchw_kernel(const uint16_t* __r
     const int c = c0 + ty + 8 * k, p = p0 + tx;
     if (c < C && p < HW) y[((size_t)b * C + c) * HW + p] = tile[tx][ty + 8 * k];
   }
-}
-
-int launch_nhwc16_to_nchw(const void* x16, float* y, int B, int C, int HW, int dtype, cudaStream_t st) {
-  HF_REQUIRE(x16 && y, "nhwc16_to_nchw: null pointer");
-  dim3 grid(cdiv_i(HW, 32), cdiv_i(C, 32), B);
-  if (dtype == HF_BF16)
-    nhwc16_to_nchw_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, y, C, HW);
-  else
-    nhwc16_to_nchw_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, y, C, HW);
-  HF_LAUNCH_OK("nhwc16_to_nchw");
-  count_launch();
-  return HF_OK;
 }
 
 // Squeeze-excite pooling (SEModule, helpers.py:57-75) in two deterministic stages.
@@ -249,15 +209,38 @@ __global__ void __launch_bounds__(256) se_gate_kernel(const float* __restrict__ 
   }
 }
 
-int channel_reduce_splits(int B, int HW, int C) {
-  const int64_t ctas = (int64_t)B * cdiv_i(C, 64);
-  int s = cdiv_i((int64_t)4 * num_sms(), ctas);
+static int channel_reduce_splits(int B, int HW, int C) {
+  const int64_t ctas = (int64_t)B * cdiv(C, 64);
+  int s = cdiv((int64_t)4 * num_sms(), ctas);
   s = std::min(s, std::max(1, HW / 64));
   return std::max(1, std::min(s, 64));
 }
 
+// stage 1 alone: ws[(b*S + s)*C + c] = partial channel sums (of (x - center)^2 with a center); *splits = S
+static int channel_partial(const void* x16, const float* center, float* ws, int B, int HW, int C, int dtype,
+                           cudaStream_t st, int* splits) {
+  HF_REQUIRE(x16 && ws && C % 8 == 0 && B > 0 && HW > 0, "channel_partial: bad arguments");
+  const int S = channel_reduce_splits(B, HW, C), chunk = cdiv(HW, S);
+  dim3 grid(cdiv(C, 64), B, S);
+  const uint16_t* x = (const uint16_t*)x16;
+  return with_dtype(dtype, "channel_partial", [&](auto dt) -> int {
+    if (center)
+      channel_sum_partial_kernel<dt, true><<<grid, 256, 0, st>>>(x, center, ws, HW, C, chunk);
+    else
+      channel_sum_partial_kernel<dt, false><<<grid, 256, 0, st>>>(x, nullptr, ws, HW, C, chunk);
+    HF_LAUNCH_OK("channel_sum_partial");
+    count_launch();
+    if (splits) *splits = S;
+    return HF_OK;
+  });
+}
+
+int launch_channel_partial(const void* x16, float* ws, int B, int HW, int C, int dtype, cudaStream_t st, int* splits) {
+  return channel_partial(x16, nullptr, ws, B, HW, C, dtype, st, splits);
+}
+
 // gate/mean [B,C] <- x16 [B,HW,C]; workspace: B * splits * C floats
-int launch_se_gate(const void* x16, const float* fc1, const float* fc2, float* out, float* ws, int B, int HW, int C,
+static int se_gate(const void* x16, const float* fc1, const float* fc2, float* out, float* ws, int B, int HW, int C,
                    int Cr, int dtype, cudaStream_t st) {
   HF_REQUIRE(x16 && out && ws, "se_gate: null pointer");
   HF_REQUIRE(C % 8 == 0 && B > 0 && HW > 0, "se_gate: channels must be a multiple of 8");
@@ -270,34 +253,6 @@ int launch_se_gate(const void* x16, const float* fc1, const float* fc2, float* o
   HF_LAUNCH_OK("se_gate");
   count_launch();
   return HF_OK;
-}
-
-// stage 1 alone: ws[(b*S + s)*C + c] = partial channel sums (of (x - center)^2 with a center); *splits = S
-static int channel_partial(const void* x16, const float* center, float* ws, int B, int HW, int C, int dtype,
-                           cudaStream_t st, int* splits) {
-  HF_REQUIRE(x16 && ws && C % 8 == 0 && B > 0 && HW > 0, "channel_partial: bad arguments");
-  const int S = channel_reduce_splits(B, HW, C), chunk = cdiv_i(HW, S);
-  dim3 grid(cdiv_i(C, 64), B, S);
-  const uint16_t* x = (const uint16_t*)x16;
-  if (center) {
-    if (dtype == HF_BF16)
-      channel_sum_partial_kernel<HF_BF16, true><<<grid, 256, 0, st>>>(x, center, ws, HW, C, chunk);
-    else
-      channel_sum_partial_kernel<HF_F16, true><<<grid, 256, 0, st>>>(x, center, ws, HW, C, chunk);
-  } else {
-    if (dtype == HF_BF16)
-      channel_sum_partial_kernel<HF_BF16, false><<<grid, 256, 0, st>>>(x, nullptr, ws, HW, C, chunk);
-    else
-      channel_sum_partial_kernel<HF_F16, false><<<grid, 256, 0, st>>>(x, nullptr, ws, HW, C, chunk);
-  }
-  HF_LAUNCH_OK("channel_sum_partial");
-  count_launch();
-  if (splits) *splits = S;
-  return HF_OK;
-}
-
-int launch_channel_partial(const void* x16, float* ws, int B, int HW, int C, int dtype, cudaStream_t st, int* splits) {
-  return channel_partial(x16, nullptr, ws, B, HW, C, dtype, st, splits);
 }
 
 // y = act((x - mean[b,c]) * rsqrt(var[b,c] + eps)), act = LeakyReLU(slope); 8 channels (16 bytes) per thread
@@ -325,37 +280,6 @@ __global__ void __launch_bounds__(256) instance_norm_apply_kernel(const uint16_t
   }
 }
 
-// InstanceNorm2d(affine=False): mean = the channel mean of launch_se_gate's two stages; var = the same two stages over
-// (x - mean)^2 (no E[x^2] - E[x]^2 cancellation); then the normalisation + LeakyReLU.  ws = [partials | mean | var].
-int launch_instance_norm_act(const void* x16, void* y16, float* ws, int B, int HW, int C, float eps, float slope,
-                             int dtype, cudaStream_t st) {
-  HF_REQUIRE(x16 && y16 && ws, "instance_norm: null pointer");
-  HF_REQUIRE(B > 0 && HW > 0 && C > 0 && C % 8 == 0, "instance_norm: bad shape B=%d HW=%d C=%d (C %% 8)", B, HW, C);
-  const int64_t total8 = (int64_t)B * HW * C / 8;
-  HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch",
-             (long long)total8);
-  const int S = channel_reduce_splits(B, HW, C);
-  float* mean = ws + (size_t)B * S * C;
-  float* var = mean + (size_t)B * C;
-  int rc = channel_partial(x16, nullptr, ws, B, HW, C, dtype, st, nullptr);
-  if (rc) return rc;
-  se_gate_kernel<<<B, 256, (size_t)C * sizeof(float), st>>>(ws, S, 1.f / (float)HW, nullptr, nullptr, mean, C, 0);
-  HF_LAUNCH_OK("instance_norm_mean");
-  if ((rc = channel_partial(x16, mean, ws, B, HW, C, dtype, st, nullptr))) return rc;
-  se_gate_kernel<<<B, 256, (size_t)C * sizeof(float), st>>>(ws, S, 1.f / (float)HW, nullptr, nullptr, var, C, 0);
-  HF_LAUNCH_OK("instance_norm_var");
-  const int grid = (int)std::min<int64_t>((total8 + 255) / 256, (int64_t)num_sms() * 16);
-  if (dtype == HF_BF16)
-    instance_norm_apply_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, mean, var, (uint16_t*)y16, HW,
-                                                              C / 8, eps, slope, (int)total8);
-  else
-    instance_norm_apply_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, mean, var, (uint16_t*)y16, HW,
-                                                             C / 8, eps, slope, (int)total8);
-  HF_LAUNCH_OK("instance_norm_apply");
-  count_launch(3);
-  return HF_OK;
-}
-
 // ReflectionPad2d(1): row / column -1 -> 1, H -> H - 2; 8 channels (16 bytes) per thread
 __global__ void __launch_bounds__(256) reflect_pad1_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int H,
                                                            int W, int C8, int total8) {
@@ -371,22 +295,6 @@ __global__ void __launch_bounds__(256) reflect_pad1_kernel(const uint4* __restri
     xi = xi < 0 ? 1 : (xi >= W ? W - 2 : xi);
     y[i] = __ldg(x + (((size_t)b * H + yi) * W + xi) * C8 + c);
   }
-}
-
-int launch_reflect_pad1(const void* x16, void* y16, int B, int H, int W, int C, int dtype, cudaStream_t st) {
-  (void)dtype;                                   // a copy: the same kernel for both 16-bit types
-  HF_REQUIRE(x16 && y16, "reflect_pad1: null pointer");
-  HF_REQUIRE(B > 0 && H >= 2 && W >= 2 && C > 0 && C % 8 == 0, "reflect_pad1: bad shape %dx%dx%d (H, W >= 2, C %% 8)",
-             H, W, C);
-  HF_REQUIRE((((uintptr_t)x16 | (uintptr_t)y16) & 15) == 0, "reflect_pad1: 16-bit tensors must be 16-byte aligned");
-  const int64_t total8 = (int64_t)B * (H + 2) * (W + 2) * C / 8;
-  HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch",
-             (long long)total8);
-  const int grid = (int)std::min<int64_t>((total8 + 255) / 256, (int64_t)num_sms() * 16);
-  reflect_pad1_kernel<<<grid, 256, 0, st>>>((const uint4*)x16, (uint4*)y16, H, W, C / 8, (int)total8);
-  HF_LAUNCH_OK("reflect_pad1");
-  count_launch();
-  return HF_OK;
 }
 
 // out = res * se[b,c] + shortcut[b, y*sc_stride, x*sc_stride, c]   (bottleneck_IR_SE.forward, helpers.py:117-120;
@@ -481,40 +389,6 @@ __global__ void __launch_bounds__(256) scale_add_vec8_kernel(const uint16_t* __r
   }
 }
 
-int launch_scale_add(const void* res16, const float* se, const void* shortcut16, int sc_stride, const float* s2,
-                     const float* b2, void* y16, void* y16b, int B, int H, int W, int C, int dtype, cudaStream_t st) {
-  HF_REQUIRE(res16 && (y16 || y16b), "scale_add: null pointer");
-  HF_REQUIRE(C % 2 == 0 && (sc_stride == 1 || sc_stride == 2), "scale_add: bad C / stride");
-  if (C % 8 == 0) {
-    const int64_t total8 = (int64_t)B * H * W * C / 8;
-    HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
-    const int grid8 = (int)std::min<int64_t>((total8 + 255) / 256, (int64_t)num_sms() * 16);
-    if (dtype == HF_BF16)
-      scale_add_vec8_kernel<HF_BF16><<<grid8, 256, 0, st>>>((const uint16_t*)res16, se, (const uint16_t*)shortcut16,
-                                                            sc_stride, s2, b2, (uint16_t*)y16, (uint16_t*)y16b, H, W,
-                                                            C / 8, total8);
-    else
-      scale_add_vec8_kernel<HF_F16><<<grid8, 256, 0, st>>>((const uint16_t*)res16, se, (const uint16_t*)shortcut16,
-                                                           sc_stride, s2, b2, (uint16_t*)y16, (uint16_t*)y16b, H, W,
-                                                           C / 8, total8);
-    HF_LAUNCH_OK("scale_add");
-    count_launch();
-    return HF_OK;
-  }
-  const int64_t total2 = (int64_t)B * H * W * C / 2;
-  HF_REQUIRE(total2 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total2);
-  const int grid = (int)std::min<int64_t>((total2 + 255) / 256, (int64_t)num_sms() * 16);
-  if (dtype == HF_BF16)
-    scale_add_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)res16, se, (const uint16_t*)shortcut16, sc_stride,
-                                                     s2, b2, (uint16_t*)y16, (uint16_t*)y16b, H, W, C, total2);
-  else
-    scale_add_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)res16, se, (const uint16_t*)shortcut16, sc_stride,
-                                                    s2, b2, (uint16_t*)y16, (uint16_t*)y16b, H, W, C, total2);
-  HF_LAUNCH_OK("scale_add");
-  count_launch();
-  return HF_OK;
-}
-
 // out = bilinear_upsample(x, size=(H,W), align_corners=True) + y   (_upsample_add, helpers.py:123-140)
 template <int DT>
 __global__ void __launch_bounds__(256) upsample_add_kernel(const uint16_t* __restrict__ x, const uint16_t* __restrict__ y,
@@ -579,37 +453,6 @@ __global__ void __launch_bounds__(256) upsample_add_vec8_kernel(const uint16_t* 
   }
 }
 
-int launch_upsample_add(const void* x16, const void* y16, void* out16, int B, int h, int w, int H, int W, int C,
-                        int dtype, cudaStream_t st) {
-  HF_REQUIRE(x16 && y16 && out16 && C % 2 == 0, "upsample_add: bad arguments");
-  if (C % 8 == 0) {
-    const int64_t total8 = (int64_t)B * H * W * C / 8;
-    HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
-    const int grid8 = (int)std::min<int64_t>((total8 + 255) / 256, (int64_t)num_sms() * 16);
-    if (dtype == HF_BF16)
-      upsample_add_vec8_kernel<HF_BF16><<<grid8, 256, 0, st>>>((const uint16_t*)x16, (const uint16_t*)y16,
-                                                               (uint16_t*)out16, h, w, H, W, C / 8, total8);
-    else
-      upsample_add_vec8_kernel<HF_F16><<<grid8, 256, 0, st>>>((const uint16_t*)x16, (const uint16_t*)y16,
-                                                              (uint16_t*)out16, h, w, H, W, C / 8, total8);
-    HF_LAUNCH_OK("upsample_add");
-    count_launch();
-    return HF_OK;
-  }
-  const int64_t total2 = (int64_t)B * H * W * C / 2;
-  HF_REQUIRE(total2 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total2);
-  const int grid = (int)std::min<int64_t>((total2 + 255) / 256, (int64_t)num_sms() * 16);
-  if (dtype == HF_BF16)
-    upsample_add_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, (const uint16_t*)y16, (uint16_t*)out16, h,
-                                                        w, H, W, C, total2);
-  else
-    upsample_add_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, (const uint16_t*)y16, (uint16_t*)out16, h, w,
-                                                       H, W, C, total2);
-  HF_LAUNCH_OK("upsample_add");
-  count_launch();
-  return HF_OK;
-}
-
 // AdaptiveAvgPool2d((oh,ow)) of an NHWC 16-bit tensor -> fp32 NCHW [B,C,oh,ow] (fs_encoder_v2, feature_style_encoder.py)
 template <int DT>
 __global__ void __launch_bounds__(256) adaptive_avgpool_kernel(const uint16_t* __restrict__ x, float* __restrict__ y,
@@ -666,29 +509,199 @@ __global__ void __launch_bounds__(256) adaptive_avgpool_vec8_kernel(const uint16
   }
 }
 
-int launch_adaptive_avgpool(const void* x16, float* y, int B, int H, int W, int C, int oh, int ow, int dtype,
-                            cudaStream_t st) {
-  HF_REQUIRE(x16 && y && oh > 0 && ow > 0, "adaptive_avgpool: bad arguments");
-  if (C % 8 == 0 && (int64_t)oh * ow <= 65535 && B <= 65535) {
-    dim3 grid(cdiv_i(C, 64), oh * ow, B);
-    if (dtype == HF_BF16)
-      adaptive_avgpool_vec8_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, y, H, W, C, oh, ow);
-    else
-      adaptive_avgpool_vec8_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, y, H, W, C, oh, ow);
+}  // namespace hf
+
+using namespace hf;
+
+extern "C" {
+
+int hf_nchw_to_nhwc16(const float* x, const float* scale, const float* shift, void* y16, int B, int C, int Cpad,
+                      int height, int width, int dtype, void* stream) {
+  return with_dtype(dtype, "hf_nchw_to_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(x && y16, "nchw_to_nhwc16: null pointer");
+    HF_REQUIRE(Cpad >= C && Cpad % 2 == 0, "nchw_to_nhwc16: bad channel padding %d for %d", Cpad, C);
+    const int HW = height * width;
+    dim3 grid(cdiv(HW, 32), cdiv(Cpad, 64), B);
+    nchw_to_nhwc16_kernel<dt><<<grid, 256, 0, (cudaStream_t)stream>>>(x, scale, shift, (uint16_t*)y16, C, Cpad, HW);
+    HF_LAUNCH_OK("nchw_to_nhwc16");
+    count_launch();
+    return HF_OK;
+  });
+}
+
+int hf_nhwc16_to_nchw(const void* x16, float* y, int B, int C, int height, int width, int dtype, void* stream) {
+  return with_dtype(dtype, "hf_nhwc16_to_nchw", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(x16 && y, "nhwc16_to_nchw: null pointer");
+    const int HW = height * width;
+    dim3 grid(cdiv(HW, 32), cdiv(C, 32), B);
+    nhwc16_to_nchw_kernel<dt><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x16, y, C, HW);
+    HF_LAUNCH_OK("nhwc16_to_nchw");
+    count_launch();
+    return HF_OK;
+  });
+}
+
+size_t hf_channel_reduce_workspace_bytes(int batch, int hw, int channels) {
+  if (batch <= 0 || hw <= 0 || channels <= 0) return 0;
+  return (size_t)batch * channel_reduce_splits(batch, hw, channels) * channels * sizeof(float);
+}
+
+size_t hf_instance_norm_workspace_bytes(int batch, int hw, int channels) {
+  if (batch <= 0 || hw <= 0 || channels <= 0) return 0;
+  return hf_channel_reduce_workspace_bytes(batch, hw, channels) + 2 * (size_t)batch * channels * sizeof(float);
+}
+
+// InstanceNorm2d(affine=False, eps 1e-5): mean = the channel mean of se_gate's two stages; var = the same two stages
+// over (x - mean)^2 (no E[x^2] - E[x]^2 cancellation); then the normalisation + LeakyReLU.  ws = [partials | mean | var].
+int hf_instance_norm_lrelu_nhwc16(const void* x16, void* y16, void* workspace, int B, int HW, int C, float slope,
+                                  int dtype, void* stream) {
+  return with_dtype(dtype, "hf_instance_norm_lrelu_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    float* ws = (float*)workspace;
+    cudaStream_t st = (cudaStream_t)stream;
+    HF_REQUIRE(x16 && y16 && ws, "instance_norm: null pointer");
+    HF_REQUIRE(B > 0 && HW > 0 && C > 0 && C % 8 == 0, "instance_norm: bad shape B=%d HW=%d C=%d (C %% 8)", B, HW, C);
+    const int64_t total8 = (int64_t)B * HW * C / 8;
+    HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch",
+               (long long)total8);
+    const int S = channel_reduce_splits(B, HW, C);
+    float* mean = ws + (size_t)B * S * C;
+    float* var = mean + (size_t)B * C;
+    if ((rc = channel_partial(x16, nullptr, ws, B, HW, C, dt, st, nullptr))) return rc;
+    se_gate_kernel<<<B, 256, (size_t)C * sizeof(float), st>>>(ws, S, 1.f / (float)HW, nullptr, nullptr, mean, C, 0);
+    HF_LAUNCH_OK("instance_norm_mean");
+    if ((rc = channel_partial(x16, mean, ws, B, HW, C, dt, st, nullptr))) return rc;
+    se_gate_kernel<<<B, 256, (size_t)C * sizeof(float), st>>>(ws, S, 1.f / (float)HW, nullptr, nullptr, var, C, 0);
+    HF_LAUNCH_OK("instance_norm_var");
+    instance_norm_apply_kernel<dt><<<grid_for(total8), 256, 0, st>>>((const uint16_t*)x16, mean, var, (uint16_t*)y16,
+                                                                     HW, C / 8, 1e-5f, slope, (int)total8);
+    HF_LAUNCH_OK("instance_norm_apply");
+    count_launch(3);
+    return HF_OK;
+  });
+}
+
+int hf_reflect_pad1_nhwc16(const void* x16, void* y16, int B, int H, int W, int C, int dtype, void* stream) {
+  // a copy: the same kernel for both 16-bit types
+  return with_dtype(dtype, "hf_reflect_pad1_nhwc16", [&](auto) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(x16 && y16, "reflect_pad1: null pointer");
+    HF_REQUIRE(B > 0 && H >= 2 && W >= 2 && C > 0 && C % 8 == 0,
+               "reflect_pad1: bad shape %dx%dx%d (H, W >= 2, C %% 8)", H, W, C);
+    HF_REQUIRE((((uintptr_t)x16 | (uintptr_t)y16) & 15) == 0, "reflect_pad1: 16-bit tensors must be 16-byte aligned");
+    const int64_t total8 = (int64_t)B * (H + 2) * (W + 2) * C / 8;
+    HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch",
+               (long long)total8);
+    reflect_pad1_kernel<<<grid_for(total8), 256, 0, (cudaStream_t)stream>>>((const uint4*)x16, (uint4*)y16, H, W, C / 8,
+                                                                            (int)total8);
+    HF_LAUNCH_OK("reflect_pad1");
+    count_launch();
+    return HF_OK;
+  });
+}
+
+int hf_channel_mean_nhwc16(const void* x16, float* mean, void* workspace, int batch, int hw, int channels, int dtype,
+                           void* stream) {
+  return with_dtype(dtype, "hf_channel_mean_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    return se_gate(x16, nullptr, nullptr, mean, (float*)workspace, batch, hw, channels, 0, dt, (cudaStream_t)stream);
+  });
+}
+
+int hf_se_gate_nhwc16(const void* x16, const float* fc1_weight, const float* fc2_weight, float* gate, void* workspace,
+                      int batch, int hw, int channels, int reduced, int dtype, void* stream) {
+  return with_dtype(dtype, "hf_se_gate_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(fc1_weight && fc2_weight, "hf_se_gate_nhwc16: null fc weights");
+    return se_gate(x16, fc1_weight, fc2_weight, gate, (float*)workspace, batch, hw, channels, reduced, dt,
+                   (cudaStream_t)stream);
+  });
+}
+
+int hf_scale_add_nhwc16(const void* res16, const float* se, const void* shortcut16, int sc_stride, const float* s2,
+                        const float* b2, void* y16, void* y16b, int B, int H, int W, int C, int dtype, void* stream) {
+  return with_dtype(dtype, "hf_scale_add_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    HF_REQUIRE(res16 && (y16 || y16b), "scale_add: null pointer");
+    HF_REQUIRE(C % 2 == 0 && (sc_stride == 1 || sc_stride == 2), "scale_add: bad C / stride");
+    if (C % 8 == 0) {
+      const int64_t total8 = (int64_t)B * H * W * C / 8;
+      HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
+      scale_add_vec8_kernel<dt><<<grid_for(total8), 256, 0, st>>>((const uint16_t*)res16, se, (const uint16_t*)shortcut16,
+                                                                  sc_stride, s2, b2, (uint16_t*)y16, (uint16_t*)y16b, H,
+                                                                  W, C / 8, total8);
+      HF_LAUNCH_OK("scale_add");
+      count_launch();
+      return HF_OK;
+    }
+    const int64_t total2 = (int64_t)B * H * W * C / 2;
+    HF_REQUIRE(total2 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total2);
+    scale_add_kernel<dt><<<grid_for(total2), 256, 0, st>>>((const uint16_t*)res16, se, (const uint16_t*)shortcut16,
+                                                           sc_stride, s2, b2, (uint16_t*)y16, (uint16_t*)y16b, H, W, C,
+                                                           total2);
+    HF_LAUNCH_OK("scale_add");
+    count_launch();
+    return HF_OK;
+  });
+}
+
+int hf_upsample_add_nhwc16(const void* x16, const void* y16, void* out16, int B, int h, int w, int H, int W, int C,
+                           int dtype, void* stream) {
+  return with_dtype(dtype, "hf_upsample_add_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    HF_REQUIRE(x16 && y16 && out16 && C % 2 == 0, "upsample_add: bad arguments");
+    if (C % 8 == 0) {
+      const int64_t total8 = (int64_t)B * H * W * C / 8;
+      HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
+      upsample_add_vec8_kernel<dt><<<grid_for(total8), 256, 0, st>>>((const uint16_t*)x16, (const uint16_t*)y16,
+                                                                     (uint16_t*)out16, h, w, H, W, C / 8, total8);
+      HF_LAUNCH_OK("upsample_add");
+      count_launch();
+      return HF_OK;
+    }
+    const int64_t total2 = (int64_t)B * H * W * C / 2;
+    HF_REQUIRE(total2 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total2);
+    upsample_add_kernel<dt><<<grid_for(total2), 256, 0, st>>>((const uint16_t*)x16, (const uint16_t*)y16,
+                                                              (uint16_t*)out16, h, w, H, W, C, total2);
+    HF_LAUNCH_OK("upsample_add");
+    count_launch();
+    return HF_OK;
+  });
+}
+
+int hf_adaptive_avgpool_nhwc16(const void* x16, float* y, int B, int H, int W, int C, int oh, int ow, int dtype,
+                               void* stream) {
+  return with_dtype(dtype, "hf_adaptive_avgpool_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    HF_REQUIRE(x16 && y && oh > 0 && ow > 0, "adaptive_avgpool: bad arguments");
+    if (C % 8 == 0 && (int64_t)oh * ow <= 65535 && B <= 65535) {
+      dim3 grid(cdiv(C, 64), oh * ow, B);
+      adaptive_avgpool_vec8_kernel<dt><<<grid, 256, 0, st>>>((const uint16_t*)x16, y, H, W, C, oh, ow);
+      HF_LAUNCH_OK("adaptive_avgpool");
+      count_launch();
+      return HF_OK;
+    }
+    const int64_t total = (int64_t)B * oh * ow * C;
+    HF_REQUIRE(total < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total);
+    adaptive_avgpool_kernel<dt><<<grid_for(total), 256, 0, st>>>((const uint16_t*)x16, y, H, W, C, oh, ow, total);
     HF_LAUNCH_OK("adaptive_avgpool");
     count_launch();
     return HF_OK;
-  }
-  const int64_t total = (int64_t)B * oh * ow * C;
-  HF_REQUIRE(total < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total);
-  const int grid = (int)std::min<int64_t>((total + 255) / 256, (int64_t)num_sms() * 16);
-  if (dtype == HF_BF16)
-    adaptive_avgpool_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, y, H, W, C, oh, ow, total);
-  else
-    adaptive_avgpool_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, y, H, W, C, oh, ow, total);
-  HF_LAUNCH_OK("adaptive_avgpool");
-  count_launch();
-  return HF_OK;
+  });
 }
 
-}  // namespace hf
+}  // extern "C"

@@ -1,8 +1,6 @@
 // Stage glue around the networks (SURVEY 8f-4): BicubicDownSample (utils/bicubic.py:6-78), the separable
 // 4*factor-tap bicubic decimation HairFast applies to every 1024^2 image (Embedding.py:66-67, Blending.py:64).
 // HBM-bound SIMT, fp32, deterministic.
-#include <algorithm>
-
 #include "hf_kernels.cuh"
 
 namespace hf {
@@ -60,23 +58,6 @@ __global__ void __launch_bounds__(256) bicubic_down_kernel(const float* __restri
   }
 }
 
-int launch_bicubic_down(const float* x, const float* k, float* y, int planes, int H, int W, int factor, int clip_round,
-                        cudaStream_t st) {
-  HF_REQUIRE(x && k && y, "bicubic_down: null pointer");
-  HF_REQUIRE(factor >= 1 && factor <= kBicMaxFactor, "bicubic_down: factor %d unsupported (1..%d)", factor, kBicMaxFactor);
-  HF_REQUIRE(planes > 0 && planes <= 65535 && H > 0 && W > 0, "bicubic_down: bad shape");
-  const int taps = 4 * factor, pad = taps - factor;
-  HF_REQUIRE(pad / 2 < H && pad - pad / 2 < H && pad / 2 < W && pad - pad / 2 < W, "bicubic_down: image smaller than the reflect padding");
-  const int Ho = (H + pad - taps) / factor + 1, Wo = (W + pad - taps) / factor + 1;
-  const size_t smem = (size_t)(4 * kBicMaxFactor + kBicTileH * (kBicTileW * factor + pad)) * sizeof(float);
-  dim3 grid((Wo + kBicTileW - 1) / kBicTileW, (Ho + kBicTileH - 1) / kBicTileH, planes);
-  bicubic_down_kernel<<<grid, 256, smem, st>>>(x, k, y, H, W, Ho, Wo, factor, clip_round);
-  HF_LAUNCH_OK("bicubic_down");
-  count_launch();
-  return HF_OK;
-}
-
-
 // ------------------------------------------------------------------------------------------------
 // DilateErosion.mask (utils/image_utils.py:42-55): `iterations` rounds of a 3x3 cross "convolution" with zero padding
 // followed by a threshold -- dilation keeps sum > 0, erosion keeps sum == 5.  One launch per round, both masks at
@@ -100,37 +81,6 @@ __global__ void __launch_bounds__(256) dilate_erode_step_kernel(const float* __r
   }
 }
 
-int launch_dilate_erode(const float* mask, float* dilate, float* erode, float* ws, int planes, int H, int W,
-                        int iterations, cudaStream_t st) {
-  HF_REQUIRE(mask && dilate && erode, "dilate_erode: null pointer");
-  HF_REQUIRE(planes > 0 && H > 0 && W > 0 && iterations >= 0, "dilate_erode: bad arguments");
-  const int64_t total = (int64_t)planes * H * W;
-  HF_REQUIRE(total < (int64_t)2000000000, "dilate_erode: tensor too large for one launch");
-  const size_t bytes = (size_t)total * sizeof(float);
-  if (iterations == 0) {
-    HF_CUDA_OK(cudaMemcpyAsync(dilate, mask, bytes, cudaMemcpyDeviceToDevice, st));
-    HF_CUDA_OK(cudaMemcpyAsync(erode, mask, bytes, cudaMemcpyDeviceToDevice, st));
-    return HF_OK;
-  }
-  HF_REQUIRE(iterations == 1 || ws, "dilate_erode: workspace (2 planes sets) needed for more than one iteration");
-  const int grid = (int)std::min<int64_t>((total + 255) / 256, (int64_t)num_sms() * 16);
-  // buffers: round r reads (d_in, e_in) and writes (d_out, e_out); the last round writes the outputs
-  const float *d_in = mask, *e_in = mask;
-  float* tmp_d[2] = {ws, ws ? ws + 2 * total : nullptr};
-  float* tmp_e[2] = {ws ? ws + total : nullptr, ws ? ws + 3 * total : nullptr};
-  for (int r = 0; r < iterations; ++r) {
-    const bool last = r == iterations - 1;
-    float* d_out = last ? dilate : tmp_d[r & 1];
-    float* e_out = last ? erode : tmp_e[r & 1];
-    dilate_erode_step_kernel<<<grid, 256, 0, st>>>(d_in, e_in, d_out, e_out, H, W, (int)total);
-    HF_LAUNCH_OK("dilate_erode_step");
-    count_launch();
-    d_in = d_out; e_in = e_out;
-  }
-  return HF_OK;
-}
-
-
 // ------------------------------------------------------------------------------------------------
 // F-space alignment (models/Alignment.py:139-159; the same blend with one stage is the Embedding mixing,
 // models/Embedding.py:86-92).
@@ -151,14 +101,6 @@ __global__ void __launch_bounds__(256) align_masks_kernel(const float* __restric
     out[n + i] = x;
     out[2 * n + i] = b * x;
   }
-}
-
-int launch_align_masks(const float* hm1, const float* hm2, const float* hmx, float* out, int n, cudaStream_t st) {
-  HF_REQUIRE(hm1 && hm2 && hmx && out && n > 0, "align_masks: bad arguments");
-  align_masks_kernel<<<(n + 255) / 256, 256, 0, st>>>(hm1, hm2, hmx, out, n);
-  HF_LAUNCH_OK("align_masks");
-  count_launch();
-  return HF_OK;
 }
 
 __device__ __forceinline__ void cubic_coeffs(float t, float* w) {
@@ -238,9 +180,82 @@ __global__ void __launch_bounds__(256) fspace_blend_kernel(const BlendArgs a) {
   }
 }
 
-int launch_fspace_blend(const float* first, const float* const* src, const float* const* mask, const float* scale_a,
+}  // namespace hf
+
+using namespace hf;
+
+extern "C" {
+
+int hf_bicubic_downsample_f32(const float* x, const float* k, float* y, int planes, int H, int W, int factor,
+                              int clip_round, void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  HF_REQUIRE(x && k && y, "bicubic_down: null pointer");
+  HF_REQUIRE(factor >= 1 && factor <= kBicMaxFactor, "bicubic_down: factor %d unsupported (1..%d)", factor, kBicMaxFactor);
+  HF_REQUIRE(planes > 0 && planes <= 65535 && H > 0 && W > 0, "bicubic_down: bad shape");
+  const int taps = 4 * factor, pad = taps - factor;
+  HF_REQUIRE(pad / 2 < H && pad - pad / 2 < H && pad / 2 < W && pad - pad / 2 < W, "bicubic_down: image smaller than the reflect padding");
+  const int Ho = (H + pad - taps) / factor + 1, Wo = (W + pad - taps) / factor + 1;
+  const size_t smem = (size_t)(4 * kBicMaxFactor + kBicTileH * (kBicTileW * factor + pad)) * sizeof(float);
+  dim3 grid((Wo + kBicTileW - 1) / kBicTileW, (Ho + kBicTileH - 1) / kBicTileH, planes);
+  bicubic_down_kernel<<<grid, 256, smem, st>>>(x, k, y, H, W, Ho, Wo, factor, clip_round);
+  HF_LAUNCH_OK("bicubic_down");
+  count_launch();
+  return HF_OK;
+}
+
+int hf_dilate_erode_f32(const float* mask, float* dilate, float* erode, void* workspace, int planes, int H, int W,
+                        int iterations, void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  HF_REQUIRE(mask && dilate && erode, "dilate_erode: null pointer");
+  HF_REQUIRE(planes > 0 && H > 0 && W > 0 && iterations >= 0, "dilate_erode: bad arguments");
+  const int64_t total = (int64_t)planes * H * W;
+  HF_REQUIRE(total < (int64_t)2000000000, "dilate_erode: tensor too large for one launch");
+  const size_t bytes = (size_t)total * sizeof(float);
+  if (iterations == 0) {
+    HF_CUDA_OK(cudaMemcpyAsync(dilate, mask, bytes, cudaMemcpyDeviceToDevice, st));
+    HF_CUDA_OK(cudaMemcpyAsync(erode, mask, bytes, cudaMemcpyDeviceToDevice, st));
+    return HF_OK;
+  }
+  HF_REQUIRE(iterations == 1 || ws, "dilate_erode: workspace (2 planes sets) needed for more than one iteration");
+  const int grid = grid_for(total);
+  // buffers: round r reads (d_in, e_in) and writes (d_out, e_out); the last round writes the outputs
+  const float *d_in = mask, *e_in = mask;
+  float* tmp_d[2] = {ws, ws ? ws + 2 * total : nullptr};
+  float* tmp_e[2] = {ws ? ws + total : nullptr, ws ? ws + 3 * total : nullptr};
+  for (int r = 0; r < iterations; ++r) {
+    const bool last = r == iterations - 1;
+    float* d_out = last ? dilate : tmp_d[r & 1];
+    float* e_out = last ? erode : tmp_e[r & 1];
+    dilate_erode_step_kernel<<<grid, 256, 0, st>>>(d_in, e_in, d_out, e_out, H, W, (int)total);
+    HF_LAUNCH_OK("dilate_erode_step");
+    count_launch();
+    d_in = d_out; e_in = e_out;
+  }
+  return HF_OK;
+}
+
+int hf_align_masks_f32(const float* hm1, const float* hm2, const float* hmx, float* out, int n, void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  HF_REQUIRE(hm1 && hm2 && hmx && out && n > 0, "align_masks: bad arguments");
+  align_masks_kernel<<<(n + 255) / 256, 256, 0, st>>>(hm1, hm2, hmx, out, n);
+  HF_LAUNCH_OK("align_masks");
+  count_launch();
+  return HF_OK;
+}
+
+int hf_fspace_blend_f32(const float* first, const float* const* src, const float* const* mask, const float* scale_a,
                         const float* scale_b, float* out, int n_stage, int C, int Ho, int Wo, int Hm, int Wm,
-                        cudaStream_t st) {
+                        void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
   HF_REQUIRE(first && src && mask && out, "fspace_blend: null pointer");
   HF_REQUIRE(n_stage >= 1 && n_stage <= kBlendMaxStage, "fspace_blend: 1..%d stages", kBlendMaxStage);
   HF_REQUIRE(C > 0 && Ho > 0 && Wo > 0 && Hm > 0 && Wm > 0, "fspace_blend: bad shape");
@@ -259,4 +274,4 @@ int launch_fspace_blend(const float* first, const float* const* src, const float
   return HF_OK;
 }
 
-}  // namespace hf
+}  // extern "C"

@@ -6,14 +6,10 @@ namespace hf {
 
 void count_launch(int n = 1);
 void reset_launch_count();
+// makes the device of hf_set_device current on this thread (no-op before the first hf_set_device)
+int ensure_device_current();
 
 // ---- hf_ops.cu : HBM-bound SIMT kernels ------------------------------------------------------
-int launch_upfirdn2d(const float* x, float* y, const float* k, int planes, int in_h, int in_w, int kh, int kw,
-                     int up_x, int up_y, int down_x, int down_y, int px0, int px1, int py0, int py1,
-                     cudaStream_t st);
-int launch_bias_act(const float* x, const float* b, float* y, int64_t n, int size_b, int64_t step_b, int act,
-                    float alpha, float scale, cudaStream_t st);
-
 struct AffineJob {      // s[b,i] = wscale * sum_j style[b, j] * mw[i,j] + mb[i]   (EqualLinear, lr_mul=1)
   const float* mw;      // [C, D]
   const float* mb;      // [C]
@@ -59,47 +55,8 @@ int launch_pack_conv2d(const float* w, const float* out_scale, void* wpk, int co
 // [4 * cout][9 * cin_pad] of the upsampling conv (row (o / 32) * 128 + parity * 32 + o % 32)
 int launch_pack_conv2d_transposed(const float* w, const float* out_scale, void* wpk, int cout, int cin, int cin_pad,
                                   int dtype, cudaStream_t st);
-// InstanceNorm2d(affine=False, eps) + LeakyReLU(slope) of x16 [B,HW,C] -> y16; ws: channel_reduce floats + 2 * B * C
-int launch_instance_norm_act(const void* x16, void* y16, float* ws, int B, int HW, int C, float eps, float slope,
-                             int dtype, cudaStream_t st);
-// ReflectionPad2d(1): x16 [B,H,W,C] -> y16 [B,H+2,W+2,C]
-int launch_reflect_pad1(const void* x16, void* y16, int B, int H, int W, int C, int dtype, cudaStream_t st);
-int launch_nchw_to_nhwc16(const float* x, const float* scale, const float* shift, void* y16, int B, int C, int Cpad,
-                          int HW, int dtype, cudaStream_t st);
-int launch_nhwc16_to_nchw(const void* x16, float* y, int B, int C, int HW, int dtype, cudaStream_t st);
-int channel_reduce_splits(int B, int HW, int C);
+// stage 1 of the deterministic channel reduction of x16 [B,HW,C]: ws[(b*S + s)*C + c] = partial sums, *splits = S
 int launch_channel_partial(const void* x16, float* ws, int B, int HW, int C, int dtype, cudaStream_t st, int* splits);
-// BiSeNet glue (hf_seg_ops.cu)
-int launch_stem7x7s2_fused(const float* x, const void* wpacked, const float* shift, void* y16, int B, int H, int W,
-                           int dtype, cudaStream_t st);
-int launch_stem3x3_fused(const float* x, const void* wpacked, const float* shift, const float* slope, const float* s2,
-                         const float* b2, void* y16, void* y16b, int B, int H, int W, int dtype, cudaStream_t st);
-int launch_maxpool3x3s2(const void* x16, void* y16, int B, int H, int W, int C, int dtype, cudaStream_t st);
-int launch_pooled_fc(const void* x16, const float* w, const float* scale, const float* shift, int act, float* out,
-                     float* ws, int B, int HW, int C, int Cout, int dtype, cudaStream_t st);
-int launch_gate_add_up(const void* x16, const float* gate, const float* addvec, const void* addt16, void* y16, int B,
-                       int h, int w, int C, int up, int dtype, cudaStream_t st);
-int launch_bicubic_down(const float* x, const float* k, float* y, int planes, int H, int W, int factor, int clip_round,
-                        cudaStream_t st);
-int launch_dilate_erode(const float* mask, float* dilate, float* erode, float* ws, int planes, int H, int W,
-                        int iterations, cudaStream_t st);
-int launch_bilinear_argmax(const float* x, long long* labels, int B, int C, int Cin, int h, int w, int H, int W,
-                           cudaStream_t st);
-int launch_align_masks(const float* hm1, const float* hm2, const float* hmx, float* out, int n, cudaStream_t st);
-int launch_fspace_blend(const float* first, const float* const* src, const float* const* mask, const float* scale_a,
-                        const float* scale_b, float* out, int n_stage, int C, int Ho, int Wo, int Hm, int Wm,
-                        cudaStream_t st);
-int launch_bilinear_up_nchw(const float* x, float* y, int B, int C, int Cin, int h, int w, int H, int W,
-                            cudaStream_t st);
-int launch_se_gate(const void* x16, const float* fc1, const float* fc2, float* out, float* ws, int B, int HW, int C,
-                   int Cr, int dtype, cudaStream_t st);
-int launch_scale_add(const void* res16, const float* se, const void* shortcut16, int sc_stride, const float* s2,
-                     const float* b2, void* y16, void* y16b, int B, int H, int W, int C, int dtype, cudaStream_t st);
-int launch_upsample_add(const void* x16, const void* y16, void* out16, int B, int h, int w, int H, int W, int C,
-                        int dtype, cudaStream_t st);
-int launch_adaptive_avgpool(const void* x16, float* y, int B, int H, int W, int C, int oh, int ow, int dtype,
-                            cudaStream_t st);
-int ensure_device_current();
 
 // ---- hf_conv_tc.cu : wgmma implicit-GEMM convolution ----------------------------------------
 struct ConvLaunch {

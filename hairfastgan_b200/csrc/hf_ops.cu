@@ -6,8 +6,6 @@
 
 namespace hf {
 
-static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
-
 // =============================================================================================
 // upfirdn2d  (reference semantics: models/stylegan2/op/upfirdn2d.py:159-200,
 //             op/upfirdn2d_kernel.cu:107-207 -- zero-stuff, pad/crop, convolve (flipped taps), decimate)
@@ -368,54 +366,6 @@ __global__ void __launch_bounds__(256) upfirdn2d_general_kernel(const float* __r
   }
 }
 
-int launch_upfirdn2d(const float* x, float* y, const float* k, int planes, int in_h, int in_w, int kh, int kw,
-                     int up_x, int up_y, int down_x, int down_y, int px0, int px1, int py0, int py1,
-                     cudaStream_t st) {
-  if (planes == 0) return HF_OK;
-  HF_REQUIRE(x && y && k, "upfirdn2d: null pointer");
-  HF_REQUIRE(planes >= 0 && in_h > 0 && in_w > 0 && kh > 0 && kw > 0, "upfirdn2d: bad shape");
-  HF_REQUIRE(up_x > 0 && up_y > 0 && down_x > 0 && down_y > 0, "upfirdn2d: up/down must be positive");
-  const int out_h = (in_h * up_y + py0 + py1 - kh) / down_y + 1;
-  const int out_w = (in_w * up_x + px0 + px1 - kw) / down_x + 1;
-  HF_REQUIRE(in_h * up_y + py0 + py1 - kh >= 0 && in_w * up_x + px0 + px1 - kw >= 0,
-             "upfirdn2d: output would be empty (in %dx%d up %d pad %d,%d k %d)", in_h, in_w, up_y, py0, py1, kh);
-  const bool k4 = (kh == 4 && kw == 4);
-  const bool sym = (up_x == up_y && down_x == down_y);
-  const bool pads03 = px0 >= 0 && py0 >= 0 && px1 >= 0 && py1 >= 0 && px0 <= 3 && px1 <= 3 && py0 <= 3 && py1 <= 3;
-  // TMA-fed strip kernels (see upfirdn2d_k4_bulk_kernel): full-width rows, 16-byte aligned tensor, pads 0..3
-  const bool bulk_ok = k4 && sym && planes <= 65535 && in_w >= 64 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
-                       ((size_t)planes * in_h * in_w) % 4 == 0;
-  auto bulk_stage = [&](int CR) {
-    return (uint32_t)((((size_t)CR * in_w * 4 + 15) / 16 * 16 + 32 + 127) / 128 * 128);
-  };
-  auto bulk_go = [&](auto kern, int rows_per_cta, int CR, int S, auto... tail) {
-    const uint32_t stage = bulk_stage(CR);                 // <= 25 KB for the widths admitted below
-    // per launch like the convolution kernels: the attribute is per device, a cache would have to be too
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-    dim3 grid(1, cdiv(up_x == 2 ? in_h : out_h, rows_per_cta), planes);
-    kern<<<grid, 256, S * stage, st>>>(x, y, k, in_h, in_w, tail..., stage);
-  };
-  if (bulk_ok && up_x == 1 && down_x == 1 && pads03 && out_w <= 1024 && in_w <= 1040) {
-    if (out_w <= 512) bulk_go(upfirdn2d_k4_bulk_kernel<1, 2, 64, 4, 3>, 64, 4, 3, out_h, out_w, px0, py0);
-    else bulk_go(upfirdn2d_k4_bulk_kernel<1, 4, 64, 4, 3>, 64, 4, 3, out_h, out_w, px0, py0);
-  } else if (bulk_ok && up_x == 1 && down_x == 2 && pads03 && out_w <= 1024 && in_w <= 1040) {
-    if (out_w <= 512) bulk_go(upfirdn2d_k4_bulk_kernel<2, 2, 32, 4, 3>, 32, 4, 3, out_h, out_w, px0, py0);
-    else bulk_go(upfirdn2d_k4_bulk_kernel<2, 4, 32, 4, 3>, 32, 4, 3, out_h, out_w, px0, py0);
-  } else if (bulk_ok && up_x == 2 && down_x == 1 && px0 == 2 && py0 == 2 && px1 == 1 && py1 == 1 && in_w <= 1024 &&
-             (reinterpret_cast<uintptr_t>(y) & 7) == 0) {
-    if (in_w <= 512) bulk_go(upfirdn2d_up2_k4_bulk_kernel<2, 32, 6, 3>, 32, 6, 3);
-    else bulk_go(upfirdn2d_up2_k4_bulk_kernel<4, 32, 6, 3>, 32, 6, 3);
-  } else {
-    int64_t total = (int64_t)planes * out_h * out_w;
-    int grid = (int)std::min<int64_t>((total + 255) / 256, (int64_t)num_sms() * 16);
-    upfirdn2d_general_kernel<<<grid, 256, 0, st>>>(x, y, k, in_h, in_w, out_h, out_w, kh, kw, up_x, up_y,
-                                                    down_x, down_y, px0, py0, total);
-  }
-  HF_LAUNCH_OK("upfirdn2d");
-  count_launch();
-  return HF_OK;
-}
-
 // =============================================================================================
 // fused bias + activation  (op/fused_bias_act_kernel.cu:19-49, forward, act in {1 linear, 3 lrelu})
 // =============================================================================================
@@ -467,35 +417,6 @@ __global__ void __launch_bounds__(256) bias_act_plane_kernel(const float* __rest
     }
     yp[i] = make_float4(r[0], r[1], r[2], r[3]);
   }
-}
-
-int launch_bias_act(const float* x, const float* b, float* y, int64_t n, int size_b, int64_t step_b, int act,
-                    float alpha, float scale, cudaStream_t st) {
-  if (n == 0) return HF_OK;
-  if (x && y && (size_b == 0 || b) && (act == 1 || act == 3) && step_b % 4 == 0 && step_b >= 1024 && n % step_b == 0 &&
-      n / step_b <= 65535 && step_b / 4 < (int64_t)2000000000 && ((((uintptr_t)x | (uintptr_t)y) & 15) == 0)) {
-    const int planes = (int)(n / step_b), quads = (int)(step_b / 4);
-    const int gx = std::max(1, std::min(cdiv(quads, 256), std::max(1, num_sms() * 16 / planes)));
-    bias_act_plane_kernel<<<dim3(gx, planes), 256, 0, st>>>(x, b, y, quads, size_b, act, alpha, scale);
-    HF_LAUNCH_OK("bias_act");
-    count_launch();
-    return HF_OK;
-  }
-  HF_REQUIRE(x && y, "bias_act: null pointer");
-  HF_REQUIRE(act == 1 || act == 3, "bias_act: act must be 1 (linear) or 3 (leaky relu), got %d", act);
-  HF_REQUIRE(n >= 0 && size_b >= 0 && step_b >= 1, "bias_act: bad sizes");
-  HF_REQUIRE(size_b == 0 || b, "bias_act: bias pointer is null");
-  if (n == 0) return HF_OK;
-  const bool vec = (step_b % 4 == 0) && (n % 4 == 0) && ((((uintptr_t)x | (uintptr_t)y) & 15) == 0);
-  int64_t work = vec ? n / 4 : n;
-  int grid = (int)std::min<int64_t>((work + 255) / 256, (int64_t)num_sms() * 16);
-  if (vec)
-    bias_act_kernel<true><<<grid, 256, 0, st>>>(x, b, y, n, size_b, step_b, act, alpha, scale);
-  else
-    bias_act_kernel<false><<<grid, 256, 0, st>>>(x, b, y, n, size_b, step_b, act, alpha, scale);
-  HF_LAUNCH_OK("bias_act");
-  count_launch();
-  return HF_OK;
 }
 
 // =============================================================================================
@@ -685,13 +606,12 @@ int launch_modulate_to_nhwc(const float* x, int x_broadcast, const float* s, con
   HF_REQUIRE(C % 2 == 0, "modulate_to_nhwc: C must be even");
   dim3 grid(cdiv(HW, 32), cdiv(C, 64), B);
   int64_t bstride = x_broadcast ? 0 : (int64_t)C * HW;
-  if (dtype == HF_BF16)
-    modulate_to_nhwc_kernel<HF_BF16><<<grid, 256, 0, st>>>(x, bstride, s, feat, alpha, (uint16_t*)xh, C, HW);
-  else
-    modulate_to_nhwc_kernel<HF_F16><<<grid, 256, 0, st>>>(x, bstride, s, feat, alpha, (uint16_t*)xh, C, HW);
-  HF_LAUNCH_OK("modulate_to_nhwc");
-  count_launch();
-  return HF_OK;
+  return with_dtype(dtype, "modulate_to_nhwc", [&](auto dt) -> int {
+    modulate_to_nhwc_kernel<dt><<<grid, 256, 0, st>>>(x, bstride, s, feat, alpha, (uint16_t*)xh, C, HW);
+    HF_LAUNCH_OK("modulate_to_nhwc");
+    count_launch();
+    return HF_OK;
+  });
 }
 
 // =============================================================================================
@@ -800,15 +720,14 @@ int launch_rgb_combine(const float* partial, int num_partials, const float* bias
   int64_t total = (int64_t)B * 3 * H * W;
   if (W % 4 == 0 && ((((uintptr_t)partial | (uintptr_t)rgb) & 15) == 0) && total / 4 < (int64_t)2000000000) {
     int64_t total4 = total / 4;
-    int grid = (int)std::min<int64_t>((total4 + 255) / 256, (int64_t)num_sms() * 16);
-    rgb_combine_vec4_kernel<<<grid, 256, 0, st>>>(partial, num_partials, total, bias, skip, up_kernel, rgb, H, W,
-                                                  total4);
+    rgb_combine_vec4_kernel<<<grid_for(total4), 256, 0, st>>>(partial, num_partials, total, bias, skip, up_kernel,
+                                                              rgb, H, W, total4);
     HF_LAUNCH_OK("rgb_combine");
     count_launch();
     return HF_OK;
   }
-  int grid = (int)std::min<int64_t>((total + 255) / 256, (int64_t)num_sms() * 16);
-  rgb_combine_kernel<<<grid, 256, 0, st>>>(partial, num_partials, total, bias, skip, up_kernel, rgb, H, W, total);
+  rgb_combine_kernel<<<grid_for(total), 256, 0, st>>>(partial, num_partials, total, bias, skip, up_kernel, rgb, H, W,
+                                                      total);
   HF_LAUNCH_OK("rgb_combine");
   count_launch();
   return HF_OK;
@@ -911,13 +830,12 @@ int launch_pack_conv(const float* w, const float* blur, void* wpk, float* wsq, i
   const float scale = 1.0f / sqrtf((float)(Cin * ksize * ksize));
   int64_t total = (int64_t)Cout * Cin;
   int grid = cdiv(total, 256);
-  if (dtype == HF_BF16)
-    pack_conv_kernel<HF_BF16><<<grid, 256, 0, st>>>(w, blur, (uint16_t*)wpk, wsq, Cout, Cin, ksize, up, scale);
-  else
-    pack_conv_kernel<HF_F16><<<grid, 256, 0, st>>>(w, blur, (uint16_t*)wpk, wsq, Cout, Cin, ksize, up, scale);
-  HF_LAUNCH_OK("pack_conv");
-  count_launch();
-  return HF_OK;
+  return with_dtype(dtype, "pack_conv", [&](auto dt) -> int {
+    pack_conv_kernel<dt><<<grid, 256, 0, st>>>(w, blur, (uint16_t*)wpk, wsq, Cout, Cin, ksize, up, scale);
+    HF_LAUNCH_OK("pack_conv");
+    count_launch();
+    return HF_OK;
+  });
 }
 
 __global__ void scale_copy_kernel(const float* __restrict__ src, float* __restrict__ dst, int64_t n, float scale) {
@@ -935,3 +853,91 @@ int launch_scale_copy(const float* src, float* dst, int64_t n, float scale, cuda
 }
 
 }  // namespace hf
+
+using namespace hf;
+
+extern "C" {
+
+int hf_upfirdn2d_f32(const float* x, float* y, const float* k, int planes, int in_h, int in_w, int kh, int kw,
+                     int up_x, int up_y, int down_x, int down_y, int px0, int px1, int py0, int py1, void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  reset_launch_count();
+  if (planes == 0) return HF_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  HF_REQUIRE(x && y && k, "upfirdn2d: null pointer");
+  HF_REQUIRE(planes >= 0 && in_h > 0 && in_w > 0 && kh > 0 && kw > 0, "upfirdn2d: bad shape");
+  HF_REQUIRE(up_x > 0 && up_y > 0 && down_x > 0 && down_y > 0, "upfirdn2d: up/down must be positive");
+  const int out_h = (in_h * up_y + py0 + py1 - kh) / down_y + 1;
+  const int out_w = (in_w * up_x + px0 + px1 - kw) / down_x + 1;
+  HF_REQUIRE(in_h * up_y + py0 + py1 - kh >= 0 && in_w * up_x + px0 + px1 - kw >= 0,
+             "upfirdn2d: output would be empty (in %dx%d up %d pad %d,%d k %d)", in_h, in_w, up_y, py0, py1, kh);
+  const bool k4 = (kh == 4 && kw == 4);
+  const bool sym = (up_x == up_y && down_x == down_y);
+  const bool pads03 = px0 >= 0 && py0 >= 0 && px1 >= 0 && py1 >= 0 && px0 <= 3 && px1 <= 3 && py0 <= 3 && py1 <= 3;
+  // TMA-fed strip kernels (see upfirdn2d_k4_bulk_kernel): full-width rows, 16-byte aligned tensor, pads 0..3
+  const bool bulk_ok = k4 && sym && planes <= 65535 && in_w >= 64 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
+                       ((size_t)planes * in_h * in_w) % 4 == 0;
+  auto bulk_stage = [&](int CR) {
+    return (uint32_t)((((size_t)CR * in_w * 4 + 15) / 16 * 16 + 32 + 127) / 128 * 128);
+  };
+  auto bulk_go = [&](auto kern, int rows_per_cta, int CR, int S, auto... tail) {
+    const uint32_t stage = bulk_stage(CR);                 // <= 25 KB for the widths admitted below
+    // per launch like the convolution kernels: the attribute is per device, a cache would have to be too
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+    dim3 grid(1, cdiv(up_x == 2 ? in_h : out_h, rows_per_cta), planes);
+    kern<<<grid, 256, S * stage, st>>>(x, y, k, in_h, in_w, tail..., stage);
+  };
+  if (bulk_ok && up_x == 1 && down_x == 1 && pads03 && out_w <= 1024 && in_w <= 1040) {
+    if (out_w <= 512) bulk_go(upfirdn2d_k4_bulk_kernel<1, 2, 64, 4, 3>, 64, 4, 3, out_h, out_w, px0, py0);
+    else bulk_go(upfirdn2d_k4_bulk_kernel<1, 4, 64, 4, 3>, 64, 4, 3, out_h, out_w, px0, py0);
+  } else if (bulk_ok && up_x == 1 && down_x == 2 && pads03 && out_w <= 1024 && in_w <= 1040) {
+    if (out_w <= 512) bulk_go(upfirdn2d_k4_bulk_kernel<2, 2, 32, 4, 3>, 32, 4, 3, out_h, out_w, px0, py0);
+    else bulk_go(upfirdn2d_k4_bulk_kernel<2, 4, 32, 4, 3>, 32, 4, 3, out_h, out_w, px0, py0);
+  } else if (bulk_ok && up_x == 2 && down_x == 1 && px0 == 2 && py0 == 2 && px1 == 1 && py1 == 1 && in_w <= 1024 &&
+             (reinterpret_cast<uintptr_t>(y) & 7) == 0) {
+    if (in_w <= 512) bulk_go(upfirdn2d_up2_k4_bulk_kernel<2, 32, 6, 3>, 32, 6, 3);
+    else bulk_go(upfirdn2d_up2_k4_bulk_kernel<4, 32, 6, 3>, 32, 6, 3);
+  } else {
+    int64_t total = (int64_t)planes * out_h * out_w;
+    upfirdn2d_general_kernel<<<grid_for(total), 256, 0, st>>>(x, y, k, in_h, in_w, out_h, out_w, kh, kw, up_x, up_y,
+                                                              down_x, down_y, px0, py0, total);
+  }
+  HF_LAUNCH_OK("upfirdn2d");
+  count_launch();
+  return HF_OK;
+}
+
+int hf_bias_act_f32(const float* x, const float* b, float* y, int64_t n, int size_b, int64_t step_b, int act,
+                    float alpha, float scale, void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  reset_launch_count();
+  if (n == 0) return HF_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (x && y && (size_b == 0 || b) && (act == 1 || act == 3) && step_b % 4 == 0 && step_b >= 1024 && n % step_b == 0 &&
+      n / step_b <= 65535 && step_b / 4 < (int64_t)2000000000 && ((((uintptr_t)x | (uintptr_t)y) & 15) == 0)) {
+    const int planes = (int)(n / step_b), quads = (int)(step_b / 4);
+    const int gx = std::max(1, std::min(cdiv(quads, 256), std::max(1, num_sms() * 16 / planes)));
+    bias_act_plane_kernel<<<dim3(gx, planes), 256, 0, st>>>(x, b, y, quads, size_b, act, alpha, scale);
+    HF_LAUNCH_OK("bias_act");
+    count_launch();
+    return HF_OK;
+  }
+  HF_REQUIRE(x && y, "bias_act: null pointer");
+  HF_REQUIRE(act == 1 || act == 3, "bias_act: act must be 1 (linear) or 3 (leaky relu), got %d", act);
+  HF_REQUIRE(n >= 0 && size_b >= 0 && step_b >= 1, "bias_act: bad sizes");
+  HF_REQUIRE(size_b == 0 || b, "bias_act: bias pointer is null");
+  if (n == 0) return HF_OK;
+  const bool vec = (step_b % 4 == 0) && (n % 4 == 0) && ((((uintptr_t)x | (uintptr_t)y) & 15) == 0);
+  const int grid = grid_for(vec ? n / 4 : n);
+  if (vec)
+    bias_act_kernel<true><<<grid, 256, 0, st>>>(x, b, y, n, size_b, step_b, act, alpha, scale);
+  else
+    bias_act_kernel<false><<<grid, 256, 0, st>>>(x, b, y, n, size_b, step_b, act, alpha, scale);
+  HF_LAUNCH_OK("bias_act");
+  count_launch();
+  return HF_OK;
+}
+
+}  // extern "C"

@@ -3,8 +3,6 @@
 // final RGB convolution.  HBM- / L2-bound SIMT, fp32 arithmetic, fixed summation orders (deterministic).
 #include <string.h>
 
-#include <algorithm>
-
 #include "hf_kernels.cuh"
 
 namespace hf {
@@ -12,24 +10,6 @@ namespace {
 
 constexpr int kClasses = 19;      // label_nc (SEAN_OPT)
 constexpr int kStyle = 512;       // ACE.style_length (normalization.py:79)
-
-template <int DT>
-__device__ __forceinline__ void ld8(const uint16_t* p, float* f) {
-  const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    f[2 * k] = Half2T<DT>::to_float((uint16_t)(w[k] & 0xFFFF));
-    f[2 * k + 1] = Half2T<DT>::to_float((uint16_t)(w[k] >> 16));
-  }
-}
-template <int DT>
-__device__ __forceinline__ void st8(uint16_t* p, const float* v) {
-  uint4 o;
-  o.x = Half2T<DT>::pack(v[0], v[1]); o.y = Half2T<DT>::pack(v[2], v[3]);
-  o.z = Half2T<DT>::pack(v[4], v[5]); o.w = Half2T<DT>::pack(v[6], v[7]);
-  *reinterpret_cast<uint4*>(p) = o;
-}
 
 // ------------------------------------------------------------------------------------------------
 // Label maps.  F.interpolate(one_hot, size=(R, R), mode='nearest') of the size^2 map picks source pixel
@@ -297,8 +277,6 @@ __global__ void __launch_bounds__(kMeanThreads) sean_class_means_kernel(const fl
   }
 }
 
-int grid_for(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, (int64_t)num_sms() * 16); }
-
 }  // namespace
 }  // namespace hf
 
@@ -321,23 +299,20 @@ int hf_sean_labels(const long long* labels, int8_t* maps, int* bad, int size, vo
 
 int hf_sean_onehot_conv(const int8_t* labels, const float* table, const float* bias, int act, void* y16, int res,
                         int channels, int dtype, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  HF_REQUIRE(labels && table && y16, "hf_sean_onehot_conv: null pointer");
-  HF_REQUIRE(res > 0 && channels > 0 && channels % 8 == 0, "hf_sean_onehot_conv: bad shape %d^2 x %d", res, channels);
-  HF_REQUIRE(act == 0 || act == 3, "hf_sean_onehot_conv: act %d (0 none, 3 ReLU)", act);
-  HF_REQUIRE(((uintptr_t)table & 15) == 0 && ((uintptr_t)y16 & 15) == 0, "hf_sean_onehot_conv: unaligned pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t total = (int64_t)res * res * (channels / 8);
-  if (dtype == HF_BF16)
-    sean_onehot_kernel<HF_BF16><<<grid_for(total), 256, 0, st>>>(labels, table, bias, act, (uint16_t*)y16, res,
-                                                                channels / 8);
-  else
-    sean_onehot_kernel<HF_F16><<<grid_for(total), 256, 0, st>>>(labels, table, bias, act, (uint16_t*)y16, res,
-                                                               channels / 8);
-  HF_LAUNCH_OK("sean_onehot");
-  count_launch();
-  return HF_OK;
+  return with_dtype(dtype, "hf_sean_onehot_conv", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(labels && table && y16, "hf_sean_onehot_conv: null pointer");
+    HF_REQUIRE(res > 0 && channels > 0 && channels % 8 == 0, "hf_sean_onehot_conv: bad shape %d^2 x %d", res, channels);
+    HF_REQUIRE(act == 0 || act == 3, "hf_sean_onehot_conv: act %d (0 none, 3 ReLU)", act);
+    HF_REQUIRE(((uintptr_t)table & 15) == 0 && ((uintptr_t)y16 & 15) == 0, "hf_sean_onehot_conv: unaligned pointer");
+    const int64_t total = (int64_t)res * res * (channels / 8);
+    sean_onehot_kernel<dt><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(labels, table, bias, act, (uint16_t*)y16,
+                                                                              res, channels / 8);
+    HF_LAUNCH_OK("sean_onehot");
+    count_launch();
+    return HF_OK;
+  });
 }
 
 int hf_sean_style_tables(const float* image_code, const float* mean_code, const hf_sean_ace_tables* aces, int n_ace,
@@ -368,25 +343,23 @@ int hf_sean_style_tables(const float* image_code, const float* mean_code, const 
 int hf_sean_ace_apply(const void* x16, const float* noise, const float* noise_var, const float* bn_scale,
                       const float* bn_shift, const float* gamma_beta, const float* table, const int8_t* labels,
                       int lrelu, void* y16, int res, int channels, int dtype, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  HF_REQUIRE(x16 && noise && noise_var && bn_scale && bn_shift && gamma_beta && y16 && (!table || labels),
-             "hf_sean_ace_apply: null pointer");
-  HF_REQUIRE(res > 0 && res * res % 32 == 0 && channels % 64 == 0 && channels > 0,
-             "hf_sean_ace_apply: bad shape %d^2 x %d (pixels %% 32, channels %% 64)", res, channels);
-  HF_REQUIRE(((uintptr_t)x16 & 15) == 0 && ((uintptr_t)y16 & 15) == 0 && ((uintptr_t)table & 15) == 0,
-             "hf_sean_ace_apply: unaligned pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  const dim3 grid(res * res / 32, channels / 64);
-  if (dtype == HF_BF16)
-    sean_ace_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, noise, noise_var, bn_scale, bn_shift,
-                                                   gamma_beta, table, labels, lrelu, (uint16_t*)y16, res, channels);
-  else
-    sean_ace_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, noise, noise_var, bn_scale, bn_shift,
-                                                  gamma_beta, table, labels, lrelu, (uint16_t*)y16, res, channels);
-  HF_LAUNCH_OK("sean_ace");
-  count_launch();
-  return HF_OK;
+  return with_dtype(dtype, "hf_sean_ace_apply", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(x16 && noise && noise_var && bn_scale && bn_shift && gamma_beta && y16 && (!table || labels),
+               "hf_sean_ace_apply: null pointer");
+    HF_REQUIRE(res > 0 && res * res % 32 == 0 && channels % 64 == 0 && channels > 0,
+               "hf_sean_ace_apply: bad shape %d^2 x %d (pixels %% 32, channels %% 64)", res, channels);
+    HF_REQUIRE(((uintptr_t)x16 & 15) == 0 && ((uintptr_t)y16 & 15) == 0 && ((uintptr_t)table & 15) == 0,
+               "hf_sean_ace_apply: unaligned pointer");
+    const dim3 grid(res * res / 32, channels / 64);
+    sean_ace_kernel<dt><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x16, noise, noise_var, bn_scale,
+                                                                bn_shift, gamma_beta, table, labels, lrelu,
+                                                                (uint16_t*)y16, res, channels);
+    HF_LAUNCH_OK("sean_ace");
+    count_launch();
+    return HF_OK;
+  });
 }
 
 int hf_sean_class_means(const float* y, const int8_t* labels, long long label_stride, float* codes, int batch,
@@ -405,20 +378,19 @@ int hf_sean_class_means(const float* y, const int8_t* labels, long long label_st
 
 int hf_sean_conv_img(const void* x16, const float* weight, const float* bias, float* y, int res, int channels,
                      int dtype, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  HF_REQUIRE(x16 && weight && bias && y, "hf_sean_conv_img: null pointer");
-  HF_REQUIRE(res > 0 && channels > 0 && channels % 8 == 0 && channels <= kImgMaxC,
-             "hf_sean_conv_img: bad shape %d^2 x %d (channels %% 8, <= %d)", res, channels, kImgMaxC);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int grid = (res * res + 255) / 256;
-  if (dtype == HF_BF16)
-    sean_conv_img_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, weight, bias, y, res, channels);
-  else
-    sean_conv_img_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, weight, bias, y, res, channels);
-  HF_LAUNCH_OK("sean_conv_img");
-  count_launch();
-  return HF_OK;
+  return with_dtype(dtype, "hf_sean_conv_img", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(x16 && weight && bias && y, "hf_sean_conv_img: null pointer");
+    HF_REQUIRE(res > 0 && channels > 0 && channels % 8 == 0 && channels <= kImgMaxC,
+               "hf_sean_conv_img: bad shape %d^2 x %d (channels %% 8, <= %d)", res, channels, kImgMaxC);
+    const int grid = (res * res + 255) / 256;
+    sean_conv_img_kernel<dt><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x16, weight, bias, y, res,
+                                                                     channels);
+    HF_LAUNCH_OK("sean_conv_img");
+    count_launch();
+    return HF_OK;
+  });
 }
 
 }  // extern "C"

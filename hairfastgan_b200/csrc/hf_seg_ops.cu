@@ -8,25 +8,6 @@
 
 namespace hf {
 
-static inline int cdiv_s(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
-
-template <int DT>
-__device__ __forceinline__ void unpack8s(const uint4& v, float* f) {
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    f[2 * k] = Half2T<DT>::to_float((uint16_t)(w[k] & 0xFFFF));
-    f[2 * k + 1] = Half2T<DT>::to_float((uint16_t)(w[k] >> 16));
-  }
-}
-template <int DT>
-__device__ __forceinline__ uint4 pack8s(const float* v) {
-  uint4 o;
-  o.x = Half2T<DT>::pack(v[0], v[1]); o.y = Half2T<DT>::pack(v[2], v[3]);
-  o.z = Half2T<DT>::pack(v[4], v[5]); o.w = Half2T<DT>::pack(v[6], v[7]);
-  return o;
-}
-
 // ------------------------------------------------------------------------------------------------
 // nn.MaxPool2d(kernel_size=3, stride=2, padding=1) (resnet.py:62,71) on NHWC 16-bit; padding never wins the max.
 // ------------------------------------------------------------------------------------------------
@@ -52,28 +33,13 @@ __global__ void __launch_bounds__(256) maxpool3x3s2_kernel(const uint16_t* __res
         const int xx = 2 * ox + dx;
         if (xx < 0 || xx >= W) continue;
         float v[8];
-        unpack8s<DT>(__ldg(reinterpret_cast<const uint4*>(x + (((size_t)b * H + yy) * W + xx) * C + c)), v);
+        unpack8<DT>(__ldg(reinterpret_cast<const uint4*>(x + (((size_t)b * H + yy) * W + xx) * C + c)), v);
 #pragma unroll
         for (int k = 0; k < 8; ++k) m[k] = fmaxf(m[k], v[k]);
       }
     }
-    *reinterpret_cast<uint4*>(y + (size_t)i * 8) = pack8s<DT>(m);
+    *reinterpret_cast<uint4*>(y + (size_t)i * 8) = pack8<DT>(m);
   }
-}
-
-int launch_maxpool3x3s2(const void* x16, void* y16, int B, int H, int W, int C, int dtype, cudaStream_t st) {
-  HF_REQUIRE(x16 && y16 && C % 8 == 0 && B > 0 && H > 0 && W > 0, "maxpool: bad arguments");
-  const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
-  const int64_t total8 = (int64_t)B * Ho * Wo * C / 8;
-  HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
-  const int grid = (int)std::min<int64_t>((total8 + 255) / 256, (int64_t)num_sms() * 16);
-  if (dtype == HF_BF16)
-    maxpool3x3s2_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, (uint16_t*)y16, H, W, Ho, Wo, C / 8, total8);
-  else
-    maxpool3x3s2_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, (uint16_t*)y16, H, W, Ho, Wo, C / 8, total8);
-  HF_LAUNCH_OK("maxpool3x3s2");
-  count_launch();
-  return HF_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -109,19 +75,6 @@ __global__ void __launch_bounds__(256) pooled_fc_kernel(const float* __restrict_
   }
 }
 
-int launch_pooled_fc(const void* x16, const float* w, const float* scale, const float* shift, int act, float* out,
-                     float* ws, int B, int HW, int C, int Cout, int dtype, cudaStream_t st) {
-  HF_REQUIRE(x16 && w && out && ws, "pooled_fc: null pointer");
-  HF_REQUIRE(C % 8 == 0 && C <= 8192 && Cout > 0 && act >= 0 && act <= 2, "pooled_fc: bad arguments");
-  int S = 1;
-  int rc = launch_channel_partial(x16, ws, B, HW, C, dtype, st, &S);
-  if (rc) return rc;
-  pooled_fc_kernel<<<B, 256, (size_t)C * sizeof(float), st>>>(ws, S, 1.f / (float)HW, w, scale, shift, act, out, C, Cout);
-  HF_LAUNCH_OK("pooled_fc");
-  count_launch();
-  return HF_OK;
-}
-
 // ------------------------------------------------------------------------------------------------
 // y[b,Y,X,c] = x[b,Y/up,X/up,c] * gate[b,c] + addvec[b,c] + addt[b,Y/up,X/up,c]      (up = 1 or 2, nearest)
 // ContextPath (model.py:116-128): feat*atten (+ the pooled branch | + the upsampled coarser branch), then
@@ -141,7 +94,7 @@ __global__ void __launch_bounds__(256) gate_add_up_kernel(const uint16_t* __rest
     const int b = (int)(t / H);
     const size_t src = (((size_t)b * h + Y / up) * w + X / up) * C + c;
     float v[8];
-    unpack8s<DT>(__ldg(reinterpret_cast<const uint4*>(x + src)), v);
+    unpack8<DT>(__ldg(reinterpret_cast<const uint4*>(x + src)), v);
     if (gate) {
 #pragma unroll
       for (int k = 0; k < 8; ++k) v[k] *= __ldg(gate + (size_t)b * C + c + k);
@@ -152,29 +105,12 @@ __global__ void __launch_bounds__(256) gate_add_up_kernel(const uint16_t* __rest
     }
     if (addt) {
       float a[8];
-      unpack8s<DT>(__ldg(reinterpret_cast<const uint4*>(addt + src)), a);
+      unpack8<DT>(__ldg(reinterpret_cast<const uint4*>(addt + src)), a);
 #pragma unroll
       for (int k = 0; k < 8; ++k) v[k] += a[k];
     }
-    *reinterpret_cast<uint4*>(y + (size_t)i * 8) = pack8s<DT>(v);
+    *reinterpret_cast<uint4*>(y + (size_t)i * 8) = pack8<DT>(v);
   }
-}
-
-int launch_gate_add_up(const void* x16, const float* gate, const float* addvec, const void* addt16, void* y16, int B,
-                       int h, int w, int C, int up, int dtype, cudaStream_t st) {
-  HF_REQUIRE(x16 && y16 && C % 8 == 0 && (up == 1 || up == 2) && B > 0 && h > 0 && w > 0, "gate_add_up: bad arguments");
-  const int64_t total8 = (int64_t)B * h * up * w * up * C / 8;
-  HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
-  const int grid = (int)std::min<int64_t>((total8 + 255) / 256, (int64_t)num_sms() * 16);
-  if (dtype == HF_BF16)
-    gate_add_up_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)x16, gate, addvec, (const uint16_t*)addt16,
-                                                      (uint16_t*)y16, h, w, up, C / 8, total8);
-  else
-    gate_add_up_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)x16, gate, addvec, (const uint16_t*)addt16,
-                                                     (uint16_t*)y16, h, w, up, C / 8, total8);
-  HF_LAUNCH_OK("gate_add_up");
-  count_launch();
-  return HF_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -191,18 +127,6 @@ constexpr int kSfRows = 8, kSfCols = 32;                 // output tile
 constexpr int kSfInRows = 2 * kSfRows + 6;               // 22 (one spare row for the zero-weight K padding)
 constexpr int kSfInPitch = 216;                          // (2*32 + 8) * 3 interleaved [x][c] 16-bit elements
 constexpr int kSfK = 176, kSfWPitch = 184;               // packed weight row: [n][k], k = ky*24 + kx*3 + c
-
-template <int DT>
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-  if (DT == HF_BF16)
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-  else
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-}
 
 template <int DT>
 __global__ void __launch_bounds__(256, 2) stem7x7s2_fused_kernel(const float* __restrict__ x,
@@ -292,8 +216,8 @@ __global__ void __launch_bounds__(256, 2) stem7x7s2_fused_kernel(const float* __
         const uint16_t* wrow = w_s + (j * 8 + g4) * kSfWPitch + ks * 16 + q2;
         bf[0] = *reinterpret_cast<const uint32_t*>(wrow);
         bf[1] = *reinterpret_cast<const uint32_t*>(wrow + 8);
-        mma16816<DT>(acc[0][j], a[0], bf);
-        mma16816<DT>(acc[1][j], a[1], bf);
+        mma16816<DT>(acc[0][j], a[0], bf[0], bf[1]);
+        mma16816<DT>(acc[1][j], a[1], bf[0], bf[1]);
       }
     }
     // ---- epilogue: + shift (BatchNorm folded: scale lives in the weights), ReLU, 16-bit, swizzled staging (its own
@@ -413,8 +337,8 @@ __global__ void __launch_bounds__(256, 2) stem3x3_fused_kernel(const float* __re
         const uint16_t* wrow = w_s + (j * 8 + g4) * kS3WPitch + ks * 16 + q2;
         bf[0] = *reinterpret_cast<const uint32_t*>(wrow);
         bf[1] = *reinterpret_cast<const uint32_t*>(wrow + 8);
-        mma16816<DT>(acc[0][j], a[0], bf);
-        mma16816<DT>(acc[1][j], a[1], bf);
+        mma16816<DT>(acc[0][j], a[0], bf[0], bf[1]);
+        mma16816<DT>(acc[1][j], a[1], bf[0], bf[1]);
       }
     }
     // ---- epilogue: v = prelu(acc + shift); pass 0 stores v, pass 1 stores v * s2 + b2 (the first block's BatchNorm)
@@ -451,53 +375,6 @@ __global__ void __launch_bounds__(256, 2) stem3x3_fused_kernel(const float* __re
       __syncthreads();                                   // out_s (and, after the last pass, in_s) may be rewritten
     }
   }
-}
-
-int launch_stem3x3_fused(const float* x, const void* wpacked, const float* shift, const float* slope, const float* s2,
-                         const float* b2, void* y16, void* y16b, int B, int H, int W, int dtype, cudaStream_t st) {
-  HF_REQUIRE(x && wpacked && shift && slope && y16, "stem3x3: null pointer");
-  HF_REQUIRE((y16b == nullptr) == (s2 == nullptr) && (s2 == nullptr) == (b2 == nullptr),
-             "stem3x3: y16b, s2 and b2 come together");
-  HF_REQUIRE(B > 0 && H > 0 && W > 0, "stem3x3: bad shape");
-  HF_REQUIRE((((uintptr_t)wpacked | (uintptr_t)y16 | (uintptr_t)y16b) & 15) == 0, "stem3x3: buffers must be 16-byte aligned");
-  const int tiles_x = cdiv_s(W, kSfCols), tiles_y = cdiv_s(H, kSfRows);
-  const int64_t total = (int64_t)tiles_x * tiles_y * B;
-  HF_REQUIRE(total < (int64_t)2000000000, "stem3x3: too many tiles");
-  const int grid = (int)std::min<int64_t>(total, (int64_t)num_sms() * 2);
-  if (dtype == HF_BF16)
-    stem3x3_fused_kernel<HF_BF16><<<grid, 256, 0, st>>>(x, (const uint16_t*)wpacked, shift, slope, s2, b2, (uint16_t*)y16,
-                                                        (uint16_t*)y16b, H, W, tiles_x, tiles_y, (int)total);
-  else
-    stem3x3_fused_kernel<HF_F16><<<grid, 256, 0, st>>>(x, (const uint16_t*)wpacked, shift, slope, s2, b2, (uint16_t*)y16,
-                                                       (uint16_t*)y16b, H, W, tiles_x, tiles_y, (int)total);
-  HF_LAUNCH_OK("stem3x3_fused");
-  count_launch();
-  return HF_OK;
-}
-
-int launch_stem7x7s2_fused(const float* x, const void* wpacked, const float* shift, void* y16, int B, int H, int W,
-                           int dtype, cudaStream_t st) {
-  HF_REQUIRE(x && wpacked && shift && y16, "stem7x7s2: null pointer");
-  HF_REQUIRE(B > 0 && H > 0 && W > 0 && B <= 65535, "stem7x7s2: bad shape");
-  HF_REQUIRE((((uintptr_t)wpacked | (uintptr_t)y16) & 15) == 0, "stem7x7s2: packed weights / output must be 16-byte aligned");
-  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-  const int tiles_x = cdiv_s(Wo, kSfCols), tiles_y = cdiv_s(Ho, kSfRows);
-  const int64_t total = (int64_t)tiles_x * tiles_y * B;
-  HF_REQUIRE(total < (int64_t)2000000000, "stem7x7s2: too many tiles");
-  const size_t smem = (size_t)(64 * kSfWPitch + kSfInRows * kSfInPitch + 256 * 64) * sizeof(uint16_t);   // 65.8 KB
-  const int grid = (int)std::min<int64_t>(total, (int64_t)num_sms() * 2);
-  if (dtype == HF_BF16) {
-    HF_CUDA_OK(cudaFuncSetAttribute(stem7x7s2_fused_kernel<HF_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    stem7x7s2_fused_kernel<HF_BF16><<<grid, 256, smem, st>>>(x, (const uint16_t*)wpacked, shift, (uint16_t*)y16, H, W, Ho,
-                                                             Wo, tiles_x, tiles_y, (int)total);
-  } else {
-    HF_CUDA_OK(cudaFuncSetAttribute(stem7x7s2_fused_kernel<HF_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    stem7x7s2_fused_kernel<HF_F16><<<grid, 256, smem, st>>>(x, (const uint16_t*)wpacked, shift, (uint16_t*)y16, H, W, Ho,
-                                                            Wo, tiles_x, tiles_y, (int)total);
-  }
-  HF_LAUNCH_OK("stem7x7s2_fused");
-  count_launch();
-  return HF_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -606,8 +483,115 @@ __global__ void __launch_bounds__(256) bilinear_argmax_kernel(const float* __res
   }
 }
 
-int launch_bilinear_argmax(const float* x, long long* labels, int B, int C, int Cin, int h, int w, int H, int W,
-                           cudaStream_t st) {
+}  // namespace hf
+
+using namespace hf;
+
+extern "C" {
+
+int hf_maxpool3x3s2_nhwc16(const void* x16, void* y16, int B, int H, int W, int C, int dtype, void* stream) {
+  return with_dtype(dtype, "hf_maxpool3x3s2_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(x16 && y16 && C % 8 == 0 && B > 0 && H > 0 && W > 0, "maxpool: bad arguments");
+    const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
+    const int64_t total8 = (int64_t)B * Ho * Wo * C / 8;
+    HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
+    maxpool3x3s2_kernel<dt><<<grid_for(total8), 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x16, (uint16_t*)y16,
+                                                                                 H, W, Ho, Wo, C / 8, total8);
+    HF_LAUNCH_OK("maxpool3x3s2");
+    count_launch();
+    return HF_OK;
+  });
+}
+
+int hf_pooled_fc_nhwc16(const void* x16, const float* w, const float* scale, const float* shift, int act, float* out,
+                        void* workspace, int B, int HW, int C, int Cout, int dtype, void* stream) {
+  return with_dtype(dtype, "hf_pooled_fc_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    float* ws = (float*)workspace;
+    cudaStream_t st = (cudaStream_t)stream;
+    HF_REQUIRE(x16 && w && out && ws, "pooled_fc: null pointer");
+    HF_REQUIRE(C % 8 == 0 && C <= 8192 && Cout > 0 && act >= 0 && act <= 2, "pooled_fc: bad arguments");
+    int S = 1;
+    if ((rc = launch_channel_partial(x16, ws, B, HW, C, dt, st, &S))) return rc;
+    pooled_fc_kernel<<<B, 256, (size_t)C * sizeof(float), st>>>(ws, S, 1.f / (float)HW, w, scale, shift, act, out, C,
+                                                                Cout);
+    HF_LAUNCH_OK("pooled_fc");
+    count_launch();
+    return HF_OK;
+  });
+}
+
+int hf_gate_add_up_nhwc16(const void* x16, const float* gate, const float* addvec, const void* addt16, void* y16,
+                          int B, int h, int w, int C, int up, int dtype, void* stream) {
+  return with_dtype(dtype, "hf_gate_add_up_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(x16 && y16 && C % 8 == 0 && (up == 1 || up == 2) && B > 0 && h > 0 && w > 0,
+               "gate_add_up: bad arguments");
+    const int64_t total8 = (int64_t)B * h * up * w * up * C / 8;
+    HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
+    gate_add_up_kernel<dt><<<grid_for(total8), 256, 0, (cudaStream_t)stream>>>(
+        (const uint16_t*)x16, gate, addvec, (const uint16_t*)addt16, (uint16_t*)y16, h, w, up, C / 8, total8);
+    HF_LAUNCH_OK("gate_add_up");
+    count_launch();
+    return HF_OK;
+  });
+}
+
+int hf_stem3x3_nhwc16(const float* x, const void* wpacked, const float* shift, const float* slope, const float* s2,
+                      const float* b2, void* y16, void* y16b, int B, int H, int W, int dtype, void* stream) {
+  return with_dtype(dtype, "hf_stem3x3_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(x && wpacked && shift && slope && y16, "stem3x3: null pointer");
+    HF_REQUIRE((y16b == nullptr) == (s2 == nullptr) && (s2 == nullptr) == (b2 == nullptr),
+               "stem3x3: y16b, s2 and b2 come together");
+    HF_REQUIRE(B > 0 && H > 0 && W > 0, "stem3x3: bad shape");
+    HF_REQUIRE((((uintptr_t)wpacked | (uintptr_t)y16 | (uintptr_t)y16b) & 15) == 0, "stem3x3: buffers must be 16-byte aligned");
+    const int tiles_x = cdiv(W, kSfCols), tiles_y = cdiv(H, kSfRows);
+    const int64_t total = (int64_t)tiles_x * tiles_y * B;
+    HF_REQUIRE(total < (int64_t)2000000000, "stem3x3: too many tiles");
+    const int grid = (int)std::min<int64_t>(total, (int64_t)num_sms() * 2);
+    stem3x3_fused_kernel<dt><<<grid, 256, 0, (cudaStream_t)stream>>>(x, (const uint16_t*)wpacked, shift, slope, s2, b2,
+                                                                     (uint16_t*)y16, (uint16_t*)y16b, H, W, tiles_x,
+                                                                     tiles_y, (int)total);
+    HF_LAUNCH_OK("stem3x3_fused");
+    count_launch();
+    return HF_OK;
+  });
+}
+
+int hf_stem7x7s2_nhwc16(const float* x, const void* wpacked, const float* shift, void* y16, int B, int H, int W,
+                        int dtype, void* stream) {
+  return with_dtype(dtype, "hf_stem7x7s2_nhwc16", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(x && wpacked && shift && y16, "stem7x7s2: null pointer");
+    HF_REQUIRE(B > 0 && H > 0 && W > 0 && B <= 65535, "stem7x7s2: bad shape");
+    HF_REQUIRE((((uintptr_t)wpacked | (uintptr_t)y16) & 15) == 0, "stem7x7s2: packed weights / output must be 16-byte aligned");
+    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+    const int tiles_x = cdiv(Wo, kSfCols), tiles_y = cdiv(Ho, kSfRows);
+    const int64_t total = (int64_t)tiles_x * tiles_y * B;
+    HF_REQUIRE(total < (int64_t)2000000000, "stem7x7s2: too many tiles");
+    const size_t smem = (size_t)(64 * kSfWPitch + kSfInRows * kSfInPitch + 256 * 64) * sizeof(uint16_t);   // 65.8 KB
+    const int grid = (int)std::min<int64_t>(total, (int64_t)num_sms() * 2);
+    HF_CUDA_OK(cudaFuncSetAttribute(stem7x7s2_fused_kernel<dt>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    stem7x7s2_fused_kernel<dt><<<grid, 256, smem, (cudaStream_t)stream>>>(x, (const uint16_t*)wpacked, shift,
+                                                                          (uint16_t*)y16, H, W, Ho, Wo, tiles_x,
+                                                                          tiles_y, (int)total);
+    HF_LAUNCH_OK("stem7x7s2_fused");
+    count_launch();
+    return HF_OK;
+  });
+}
+
+int hf_bilinear_argmax_nchw_f32(const float* x, long long* labels, int B, int C, int Cin, int h, int w, int H, int W,
+                                void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
   HF_REQUIRE(x && labels && B > 0 && C > 0 && Cin >= C && h > 0 && w > 0 && H > 0 && W > 0,
              "bilinear_argmax: bad arguments");
   const size_t smem = (size_t)C * w * sizeof(float);
@@ -617,17 +601,20 @@ int launch_bilinear_argmax(const float* x, long long* labels, int B, int C, int 
   if (smem > 48 * 1024)
     HF_CUDA_OK(cudaFuncSetAttribute(bilinear_argmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = (int)std::min<int64_t>(rows, (int64_t)num_sms() * 8);
-  bilinear_argmax_kernel<<<grid, 256, smem, st>>>(x, labels, C, Cin, h, w, H, W, (int)rows);
+  bilinear_argmax_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(x, labels, C, Cin, h, w, H, W, (int)rows);
   HF_LAUNCH_OK("bilinear_argmax");
   count_launch();
   return HF_OK;
 }
 
-int launch_bilinear_up_nchw(const float* x, float* y, int B, int C, int Cin, int h, int w, int H, int W,
-                            cudaStream_t st) {
+int hf_bilinear_upsample_nchw_f32(const float* x, float* y, int B, int C, int Cin, int h, int w, int H, int W,
+                                  void* stream) {
+  int rc = ensure_device_current();
+  if (rc) return rc;
   HF_REQUIRE(x && y && B > 0 && C > 0 && Cin >= C && h > 0 && w > 0 && H > 0 && W > 0, "bilinear_up: bad arguments");
   const int64_t total = (int64_t)B * C * H * W;
   HF_REQUIRE(total < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total);
+  cudaStream_t st = (cudaStream_t)stream;
   if (W % 4 == 0 && (((uintptr_t)y) & 15) == 0 && w <= 8192) {
     const int64_t rows = (int64_t)B * C * H;
     const int grid = (int)std::min<int64_t>(rows, (int64_t)num_sms() * 16);
@@ -641,4 +628,4 @@ int launch_bilinear_up_nchw(const float* x, float* y, int B, int C, int Cin, int
   return HF_OK;
 }
 
-}  // namespace hf
+}  // extern "C"

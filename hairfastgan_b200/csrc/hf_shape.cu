@@ -14,27 +14,6 @@ constexpr int kOutClasses = 19;
 constexpr int kHairIdx = 13;      // HAIR_IDX (global_value_utils.py:52)
 constexpr int kOutC = 32;         // channels of both decoders' last LayerNorm layer
 
-template <int DT>
-__device__ __forceinline__ void ld8(const uint16_t* p, float* f) {
-  const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    f[2 * k] = Half2T<DT>::to_float((uint16_t)(w[k] & 0xFFFF));
-    f[2 * k + 1] = Half2T<DT>::to_float((uint16_t)(w[k] >> 16));
-  }
-}
-template <int DT>
-__device__ __forceinline__ void st8(uint16_t* p, const float* v) {
-  uint4 o;
-  o.x = Half2T<DT>::pack(v[0], v[1]); o.y = Half2T<DT>::pack(v[2], v[3]);
-  o.z = Half2T<DT>::pack(v[4], v[5]); o.w = Half2T<DT>::pack(v[6], v[7]);
-  *reinterpret_cast<uint4*>(p) = o;
-}
-
-int cdiv_i(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
-int grid_for(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, (int64_t)num_sms() * 16); }
-
 // ------------------------------------------------------------------------------------------------
 // Label map.  mask_label_to_one_hot (shape_util.py:6-14) rewrites 255 -> 19 in the caller's long tensor and scatters
 // into 20 channels, dropping the last: 19 is the all-zero one-hot.  Labels outside {0..19, 255} are counted in *bad
@@ -95,18 +74,6 @@ __global__ void __launch_bounds__(256) shape_onehot_s2_kernel(const int8_t* __re
 // 4-stage cp.async ring (zero fill outside the image and beyond K), XOR-swizzled 128-byte shared-memory rows.
 // ------------------------------------------------------------------------------------------------
 constexpr int kGemmBM = 128, kGemmBK = 64, kGemmStages = 4, kGemmThreads = 128, kGemmMinKt = 4;
-
-template <int DT>
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  if (DT == HF_BF16)
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-  else
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(bytes) : "memory");
@@ -395,8 +362,8 @@ int gemm_shape(int mode, int cin, int hin, int win, GemmShape* g) {
 // {BN, splits, k tiles, grid m, grid n}: enough splits for two CTAs per SM, at least kGemmMinKt k tiles per split
 void gemm_plan(const GemmShape& g, int cout, int sms, int* out) {
   const int bn = g.P <= 8 ? 8 : 64;
-  const int gm = cdiv_i(cout, kGemmBM), gn = cdiv_i(g.P, bn), kt = cdiv_i(g.K, kGemmBK);
-  const int splits = std::max(1, std::min(cdiv_i(2 * sms, gm * gn), kt / kGemmMinKt));
+  const int gm = cdiv(cout, kGemmBM), gn = cdiv(g.P, bn), kt = cdiv(g.K, kGemmBK);
+  const int splits = std::max(1, std::min(cdiv(2 * sms, gm * gn), kt / kGemmMinKt));
   out[0] = bn; out[1] = splits; out[2] = kt; out[3] = gm; out[4] = gn;
 }
 
@@ -447,23 +414,20 @@ int hf_shape_labels(long long* mask, int8_t* labels, int* bad, int n, void* stre
 
 int hf_shape_onehot_s2(const int8_t* labels, const float* table, const float* cmap, void* y16, int res, int channels,
                        int dtype, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  HF_REQUIRE(labels && table && cmap && y16, "hf_shape_onehot_s2: null pointer");
-  HF_REQUIRE(res > 0 && channels > 0 && channels % 8 == 0, "hf_shape_onehot_s2: bad shape %d^2 x %d", res, channels);
-  HF_REQUIRE(((uintptr_t)table & 15) == 0 && ((uintptr_t)cmap & 15) == 0 && ((uintptr_t)y16 & 15) == 0,
-             "hf_shape_onehot_s2: unaligned pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t total = (int64_t)res * res * (channels / 8);
-  if (dtype == HF_BF16)
-    shape_onehot_s2_kernel<HF_BF16><<<grid_for(total), 256, 0, st>>>(labels, table, cmap, (uint16_t*)y16, res,
-                                                                    channels / 8);
-  else
-    shape_onehot_s2_kernel<HF_F16><<<grid_for(total), 256, 0, st>>>(labels, table, cmap, (uint16_t*)y16, res,
-                                                                   channels / 8);
-  HF_LAUNCH_OK("shape_onehot_s2");
-  count_launch();
-  return HF_OK;
+  return with_dtype(dtype, "hf_shape_onehot_s2", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(labels && table && cmap && y16, "hf_shape_onehot_s2: null pointer");
+    HF_REQUIRE(res > 0 && channels > 0 && channels % 8 == 0, "hf_shape_onehot_s2: bad shape %d^2 x %d", res, channels);
+    HF_REQUIRE(((uintptr_t)table & 15) == 0 && ((uintptr_t)cmap & 15) == 0 && ((uintptr_t)y16 & 15) == 0,
+               "hf_shape_onehot_s2: unaligned pointer");
+    const int64_t total = (int64_t)res * res * (channels / 8);
+    shape_onehot_s2_kernel<dt><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(labels, table, cmap, (uint16_t*)y16,
+                                                                                  res, channels / 8);
+    HF_LAUNCH_OK("shape_onehot_s2");
+    count_launch();
+    return HF_OK;
+  });
 }
 
 int hf_shape_gemm_plan(int mode, int cin, int cout, int hin, int win, int sms, int* out) {
@@ -485,35 +449,28 @@ size_t hf_shape_gemm_workspace_bytes(int mode, int cin, int cout, int hin, int w
 
 int hf_shape_gemm(int mode, const void* w16, const void* x16, const float* bias, float* y32, void* y16, float* workspace,
                   int cin, int cout, int hin, int win, int dtype, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  HF_REQUIRE(w16 && x16 && workspace && (y32 || y16), "hf_shape_gemm: null pointer");
-  HF_REQUIRE(((uintptr_t)w16 & 15) == 0 && ((uintptr_t)x16 & 15) == 0, "hf_shape_gemm: unaligned operand");
-  HF_REQUIRE(cout > 0, "hf_shape_gemm: cout %d", cout);
-  GemmShape g;
-  if ((rc = gemm_shape(mode, cin, hin, win, &g))) return rc;
-  int pl[5];
-  gemm_plan(g, cout, num_sms(), pl);
-  cudaStream_t st = (cudaStream_t)stream;
-  const uint16_t* w = (const uint16_t*)w16;
-  const uint16_t* x = (const uint16_t*)x16;
-  if (dtype == HF_BF16)
-    rc = pl[0] == 8 ? launch_gemm_mode<HF_BF16, 8>(mode, w, x, workspace, cout, g, pl, cin, st)
-                    : launch_gemm_mode<HF_BF16, 64>(mode, w, x, workspace, cout, g, pl, cin, st);
-  else
-    rc = pl[0] == 8 ? launch_gemm_mode<HF_F16, 8>(mode, w, x, workspace, cout, g, pl, cin, st)
-                    : launch_gemm_mode<HF_F16, 64>(mode, w, x, workspace, cout, g, pl, cin, st);
-  if (rc) return rc;
-  const int64_t n = (int64_t)g.P * cout;
-  if (dtype == HF_BF16)
-    shape_splitk_reduce_kernel<HF_BF16><<<grid_for(n), 256, 0, st>>>(workspace, pl[1], n, cout, bias, y32,
-                                                                    (uint16_t*)y16);
-  else
-    shape_splitk_reduce_kernel<HF_F16><<<grid_for(n), 256, 0, st>>>(workspace, pl[1], n, cout, bias, y32,
-                                                                   (uint16_t*)y16);
-  HF_LAUNCH_OK("shape_splitk_reduce");
-  count_launch(2);
-  return HF_OK;
+  return with_dtype(dtype, "hf_shape_gemm", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(w16 && x16 && workspace && (y32 || y16), "hf_shape_gemm: null pointer");
+    HF_REQUIRE(((uintptr_t)w16 & 15) == 0 && ((uintptr_t)x16 & 15) == 0, "hf_shape_gemm: unaligned operand");
+    HF_REQUIRE(cout > 0, "hf_shape_gemm: cout %d", cout);
+    GemmShape g;
+    if ((rc = gemm_shape(mode, cin, hin, win, &g))) return rc;
+    int pl[5];
+    gemm_plan(g, cout, num_sms(), pl);
+    cudaStream_t st = (cudaStream_t)stream;
+    const uint16_t* w = (const uint16_t*)w16;
+    const uint16_t* x = (const uint16_t*)x16;
+    rc = pl[0] == 8 ? launch_gemm_mode<dt, 8>(mode, w, x, workspace, cout, g, pl, cin, st)
+                    : launch_gemm_mode<dt, 64>(mode, w, x, workspace, cout, g, pl, cin, st);
+    if (rc) return rc;
+    const int64_t n = (int64_t)g.P * cout;
+    shape_splitk_reduce_kernel<dt><<<grid_for(n), 256, 0, st>>>(workspace, pl[1], n, cout, bias, y32, (uint16_t*)y16);
+    HF_LAUNCH_OK("shape_splitk_reduce");
+    count_launch(2);
+    return HF_OK;
+  });
 }
 
 size_t hf_shape_layer_norm_workspace_bytes(long long n) {
@@ -523,53 +480,48 @@ size_t hf_shape_layer_norm_workspace_bytes(long long n) {
 
 int hf_shape_layer_norm_lrelu(const void* x16, const float* gamma, const float* beta, void* y16, float* workspace,
                               int pixels, int channels, float slope, int dtype, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  HF_REQUIRE(x16 && gamma && beta && y16 && workspace, "hf_shape_layer_norm_lrelu: null pointer");
-  HF_REQUIRE(pixels > 0 && channels > 0 && channels % 8 == 0 && (int64_t)pixels * channels > 1,
-             "hf_shape_layer_norm_lrelu: bad shape %d x %d (channels %% 8)", pixels, channels);
-  HF_REQUIRE(((uintptr_t)x16 & 15) == 0 && ((uintptr_t)y16 & 15) == 0, "hf_shape_layer_norm_lrelu: unaligned pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t n8 = (int64_t)pixels * channels / 8;
-  const int G = ln_blocks(n8);
-  const int64_t chunk8 = (n8 + G - 1) / G;
-  float* sums = workspace;
-  float* sqsums = workspace + G;
-  const uint16_t* x = (const uint16_t*)x16;
-  if (dtype == HF_BF16) {
-    shape_ln_partial_kernel<HF_BF16, false><<<G, kLnThreads, 0, st>>>(x, n8, chunk8, nullptr, G, sums);
-    shape_ln_partial_kernel<HF_BF16, true><<<G, kLnThreads, 0, st>>>(x, n8, chunk8, sums, G, sqsums);
-    shape_ln_apply_kernel<HF_BF16><<<grid_for(n8), kLnThreads, 0, st>>>(x, sums, sqsums, G, n8, channels / 8, gamma,
-                                                                       beta, 1e-5f, slope, (uint16_t*)y16);
-  } else {
-    shape_ln_partial_kernel<HF_F16, false><<<G, kLnThreads, 0, st>>>(x, n8, chunk8, nullptr, G, sums);
-    shape_ln_partial_kernel<HF_F16, true><<<G, kLnThreads, 0, st>>>(x, n8, chunk8, sums, G, sqsums);
-    shape_ln_apply_kernel<HF_F16><<<grid_for(n8), kLnThreads, 0, st>>>(x, sums, sqsums, G, n8, channels / 8, gamma,
-                                                                      beta, 1e-5f, slope, (uint16_t*)y16);
-  }
-  HF_LAUNCH_OK("shape_layer_norm");
-  count_launch(3);
-  return HF_OK;
+  return with_dtype(dtype, "hf_shape_layer_norm_lrelu", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(x16 && gamma && beta && y16 && workspace, "hf_shape_layer_norm_lrelu: null pointer");
+    HF_REQUIRE(pixels > 0 && channels > 0 && channels % 8 == 0 && (int64_t)pixels * channels > 1,
+               "hf_shape_layer_norm_lrelu: bad shape %d x %d (channels %% 8)", pixels, channels);
+    HF_REQUIRE(((uintptr_t)x16 & 15) == 0 && ((uintptr_t)y16 & 15) == 0,
+               "hf_shape_layer_norm_lrelu: unaligned pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t n8 = (int64_t)pixels * channels / 8;
+    const int G = ln_blocks(n8);
+    const int64_t chunk8 = (n8 + G - 1) / G;
+    float* sums = workspace;
+    float* sqsums = workspace + G;
+    const uint16_t* x = (const uint16_t*)x16;
+    shape_ln_partial_kernel<dt, false><<<G, kLnThreads, 0, st>>>(x, n8, chunk8, nullptr, G, sums);
+    shape_ln_partial_kernel<dt, true><<<G, kLnThreads, 0, st>>>(x, n8, chunk8, sums, G, sqsums);
+    shape_ln_apply_kernel<dt><<<grid_for(n8), kLnThreads, 0, st>>>(x, sums, sqsums, G, n8, channels / 8, gamma, beta,
+                                                                   1e-5f, slope, (uint16_t*)y16);
+    HF_LAUNCH_OK("shape_layer_norm");
+    count_launch(3);
+    return HF_OK;
+  });
 }
 
 int hf_shape_logits_argmax(const void* hair16, const void* face16, const float* table, const float* bias,
                            long long* labels, int res, int dtype, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  HF_REQUIRE(hair16 && face16 && table && bias && labels, "hf_shape_logits_argmax: null pointer");
-  HF_REQUIRE(res > 0 && res <= 4096, "hf_shape_logits_argmax: res %d", res);
-  HF_REQUIRE(((uintptr_t)hair16 & 15) == 0 && ((uintptr_t)face16 & 15) == 0, "hf_shape_logits_argmax: unaligned input");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int grid = (res * res + 255) / 256;
-  if (dtype == HF_BF16)
-    shape_logits_argmax_kernel<HF_BF16><<<grid, 256, 0, st>>>((const uint16_t*)hair16, (const uint16_t*)face16, table,
-                                                              bias, labels, res);
-  else
-    shape_logits_argmax_kernel<HF_F16><<<grid, 256, 0, st>>>((const uint16_t*)hair16, (const uint16_t*)face16, table,
-                                                             bias, labels, res);
-  HF_LAUNCH_OK("shape_logits_argmax");
-  count_launch();
-  return HF_OK;
+  return with_dtype(dtype, "hf_shape_logits_argmax", [&](auto dt) -> int {
+    int rc = ensure_device_current();
+    if (rc) return rc;
+    HF_REQUIRE(hair16 && face16 && table && bias && labels, "hf_shape_logits_argmax: null pointer");
+    HF_REQUIRE(res > 0 && res <= 4096, "hf_shape_logits_argmax: res %d", res);
+    HF_REQUIRE(((uintptr_t)hair16 & 15) == 0 && ((uintptr_t)face16 & 15) == 0,
+               "hf_shape_logits_argmax: unaligned input");
+    const int grid = (res * res + 255) / 256;
+    shape_logits_argmax_kernel<dt><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)hair16,
+                                                                           (const uint16_t*)face16, table, bias,
+                                                                           labels, res);
+    HF_LAUNCH_OK("shape_logits_argmax");
+    count_launch();
+    return HF_OK;
+  });
 }
 
 }  // extern "C"

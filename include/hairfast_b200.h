@@ -26,7 +26,8 @@ extern "C" {
 #define HF_ERR_CUDA (-2)        /* CUDA runtime / driver error */
 #define HF_ERR_UNSUPPORTED (-3) /* device is not sm_90 */
 
-/* 16-bit storage/operand type of the tensor-core path (accumulation is always fp32) */
+/* 16-bit storage/operand type of the tensor-core path (accumulation is always fp32).  A call that takes an
+ * `int dtype` returns HF_ERR_INVALID for any other value, before it checks its other arguments. */
 #define HF_BF16 0
 #define HF_F16 1
 

@@ -58,6 +58,25 @@ def test_argument_validation_without_device(lib):
     assert h.hf_upfirdn2d_f32(None, None, None, 0, 4, 4, 4, 4, 1, 1, 1, 1, 0, 0, 0, 0, None) == 0   # empty input
 
 
+def test_every_dtype_argument_is_checked_first(lib):
+    """Every call with an `int dtype` parameter rejects a value other than HF_BF16 / HF_F16 before its other
+    argument checks: with every other argument zero / NULL the error names the dtype."""
+    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "hairfast_b200.h")).read(), flags=re.S)
+    dtype_pos = {}
+    for name, params in re.findall(r"\b(hf_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", hdr):
+        if re.search(r"\bint\s+dtype\b", params):
+            dtype_pos[name] = [re.findall(r"\w+", p)[-1] for p in params.split(",")].index("dtype")
+    assert len(dtype_pos) == 21, sorted(dtype_pos)
+    h = lib.lib()
+    for name, pos in sorted(dtype_pos.items()):
+        argtypes = lib.SYMBOLS[name][1]
+        for bad in (2, -1):
+            args = [None if t is C.c_void_p or issubclass(t, C._Pointer) else t(0) for t in argtypes]
+            args[pos] = bad
+            assert getattr(h, name)(*args) == -1, name               # HF_ERR_INVALID
+            assert h.hf_last_error() == f"{name}: bad dtype {bad}".encode(), (name, h.hf_last_error())
+
+
 def test_module_surface_matches_reference_signatures():
     """Same ctor / forward parameter names and defaults as models/stylegan2/model.py (SURVEY 8b)."""
     import hairfastgan_b200.model as M
