@@ -1,7 +1,7 @@
 """One process = one arm of the full `HairFast.swap()` comparison (BASELINE configs[2], SURVEY 8d config 3).
 
-    python baseline/run_swap.py --mode reference|overlay|overlay_fast|overlay_sean|overlay_sean_full|overlay_all --work DIR
-                                --out result.pt [--reps N]
+    python baseline/run_swap.py --mode reference|overlay|overlay_fast|overlay_sean|overlay_sean_full|overlay_all|
+                                       overlay_modulation --work DIR --out result.pt [--reps N]
 
 * reference     the unmodified reference (oracle/_ref): cuDNN grouped convolutions + its two JIT kernels, fp32/TF32
 * overlay       the same checkout with hairfastgan_b200.install() active (this package's modules under its names)
@@ -9,6 +9,8 @@
 * overlay_sean  overlay + install(sean=True): SEAN's decode_sean on hairfastgan_b200/sean.py
 * overlay_sean_full  overlay + install(sean=True, sean_encode=True): SEAN's encode_sean and decode_sean on it
 * overlay_all        overlay_sean_full + install(shape_adaptor=True): CtrlHair's shape adaptor on it too
+* overlay_modulation overlay_all + install(modulation=True): HairFast's Rotate / Blending / PostProcess latent
+                     modulation stacks on it too
 
 Three synthetic images `torch.rand(3,1024,1024)` (seeds 0,1,2) are passed as tensors (hair_swap.py:63-105), synthetic
 checkpoints come from baseline/synth_checkpoints.py, `swap(..., seed=3407)` is the default seed (utils/seed.py:22-28).
@@ -33,7 +35,7 @@ from baseline import refenv, synth_checkpoints  # noqa: E402
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--mode", choices=["reference", "overlay", "overlay_fast", "overlay_sean", "overlay_sean_full",
-                                       "overlay_all"],
+                                       "overlay_all", "overlay_modulation"],
                     required=True)
     ap.add_argument("--work", default="/tmp/hairfast_work")
     ap.add_argument("--out", default=None)
@@ -50,7 +52,9 @@ def main():
         subprocess.run([sys.executable, os.path.join(HERE, "synth_checkpoints.py"), work], check=True)
 
     sean = {"overlay_sean": {"sean": True}, "overlay_sean_full": {"sean": True, "sean_encode": True},
-            "overlay_all": {"sean": True, "sean_encode": True, "shape_adaptor": True}}.get(a.mode, {})
+            "overlay_all": {"sean": True, "sean_encode": True, "shape_adaptor": True},
+            "overlay_modulation": {"sean": True, "sean_encode": True, "shape_adaptor": True,
+                                   "modulation": True}}.get(a.mode, {})
     refenv.activate(overlay=a.mode != "reference", skip_fse_reconstruction=a.mode == "overlay_fast", workdir=work,
                     **sean)
     import torch

@@ -49,6 +49,14 @@ class hf_sean_ace_tables(C.Structure):
     _fields_ = [("fc_w", C.c_void_p), ("fc_b", C.c_void_p), ("tw", C.c_void_p), ("table", C.c_void_p), ("n2", C.c_int)]
 
 
+class hf_mod_desc(C.Structure):
+    _fields_ = [("layers", C.c_int), ("inp", C.c_int), ("middle", C.c_int), ("stacks", C.c_int), ("dtype", C.c_int)]
+
+
+class hf_mod_rows(C.Structure):
+    _fields_ = [("ptr", C.c_void_p), ("batch_stride", C.c_longlong), ("row_stride", C.c_longlong)]
+
+
 class hf_gen_config(C.Structure):
     _fields_ = [("size", C.c_int), ("style_dim", C.c_int), ("channel_multiplier", C.c_int), ("dtype", C.c_int)]
 
@@ -161,6 +169,13 @@ SYMBOLS = {
     "hf_shape_layer_norm_lrelu": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p]),
     "hf_shape_layer_norm_workspace_bytes": (C.c_size_t, [C.c_longlong]),
     "hf_shape_logits_argmax": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_void_p]),
+    "hf_mod_workspace_bytes": (C.c_size_t, [C.POINTER(hf_mod_desc), C.c_int]),
+    "hf_mod_gemm_plan": (C.c_int, [C.POINTER(hf_mod_desc), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]),
+    "hf_mod_embed16": (C.c_int, [C.POINTER(hf_mod_desc), C.c_int, C.POINTER(hf_mod_rows), C.c_void_p, C.c_void_p]),
+    "hf_mod_gemm": (C.c_int, [C.POINTER(hf_mod_desc), C.c_int, C.c_int] + [C.c_void_p] * 6),
+    "hf_mod_hidden": (C.c_int, [C.POINTER(hf_mod_desc), C.c_int] + [C.c_void_p] * 8),
+    "hf_mod_chain": (C.c_int, [C.POINTER(hf_mod_desc), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.POINTER(hf_mod_rows), C.POINTER(hf_mod_rows), C.c_void_p, C.c_void_p, C.c_void_p]),
     "hf_generator_packed_bytes":(C.c_size_t, [C.POINTER(hf_gen_config)]),
     "hf_generator_workspace_bytes": (C.c_size_t, [C.POINTER(hf_gen_config), C.c_int]),
     "hf_generator_pack": (C.c_int, [C.POINTER(hf_gen_config), C.POINTER(hf_gen_weights), C.c_void_p, C.c_void_p]),

@@ -41,6 +41,9 @@ After ``install()`` the import statements of the reference resolve to this packa
 * opt-in, ``install(shape_adaptor=True)``: CtrlHair's ``get_hair_face_code`` and ``get_new_shape``
   (models/CtrlHair/shape_branch/solver.py:248-262) are rebound inside that module and ``models.Alignment`` (which
   imports both names, Alignment.py:7)                                               -> ``hairfastgan_b200.shape_adaptor``
+* opt-in, ``install(modulation=True)``: ``RotateModel.forward``, ``ClipBlendingModel.forward`` and
+  ``PostProcessModel.forward`` (models/Encoders.py:66-137) are wrapped inside ``models.Encoders`` after import; the
+  classes, their submodules and state-dict keys stay the reference's             -> ``hairfastgan_b200.modulation``
 
 Nothing in the reference tree is edited and its JIT build of the two 2019 CUDA extensions
 (op/fused_act.py:10-16, op/upfirdn2d.py:10-16) never runs.
@@ -109,6 +112,10 @@ _sean_names = set()
 _sean_saved = {}
 _post_import = set()          # module names the meta-path hook currently patches
 _patched_trainers = []
+# HairFast's modulation nets (opt-in): the forwards of three classes in models/Encoders.py are wrapped after import
+_MODULATION_MODULE = "models.Encoders"
+_options = {"postprocess": False, "modulation": False}
+_patched_modulation = []
 
 
 def _patch_sean(module, name: str) -> None:
@@ -141,7 +148,12 @@ def _patch_postprocess(module) -> None:
         if fast.patch_trainer_module(module):
             _patched_trainers.append(module)
         return
-    rebind = [(attr, "hairfastgan_b200.postprocess") for attr in _POSTPROCESS.get(module.__name__, ())]
+    if module.__name__ == _MODULATION_MODULE and _options["modulation"]:
+        mod = importlib.import_module("hairfastgan_b200.modulation")
+        if mod.patch_encoders_module(module):
+            _patched_modulation.append(module)
+    rebind = [(attr, "hairfastgan_b200.postprocess") for attr in _POSTPROCESS.get(module.__name__, ())
+              if _options["postprocess"]]
     rebind += list(_GLUE_ATTRS.get(module.__name__, ()))
     for attr, ours_name in rebind:
         ours = importlib.import_module(ours_name)
@@ -203,13 +215,16 @@ def _register(ref_name: str, ours: str) -> None:
 
 def install(generator: bool = True, encoders: bool = True, postprocess: bool = True, segmentation: bool = True,
             glue: bool = True, skip_fse_reconstruction: bool = False, fuse_face_parsing: bool = True,
-            sean: bool = False, sean_encode: bool = False, shape_adaptor: bool = False) -> None:
+            sean: bool = False, sean_encode: bool = False, shape_adaptor: bool = False,
+            modulation: bool = False) -> None:
     """Register the overlay.  ``generator=False`` swaps only the operator package (L1 boundary) and leaves the
     reference's own ``models/stylegan2/model.py`` classes in place on top of our ops; ``encoders=False`` keeps
     the reference's PyTorch encoders; ``postprocess=False`` keeps its PostProcess conv stack; ``segmentation=False``
     its BiSeNet.  ``sean=True`` (off by default) runs SEAN's ``decode_sean`` on our kernels; ``sean_encode=True`` (off
     by default, independent of ``sean``) runs its ``encode_sean`` (the Zencoder) on them; ``shape_adaptor=True`` (off by
-    default) runs CtrlHair's shape adaptor (``get_hair_face_code`` / ``get_new_shape``) on them."""
+    default) runs CtrlHair's shape adaptor (``get_hair_face_code`` / ``get_new_shape``) on them; ``modulation=True``
+    (off by default, independent of ``postprocess``) runs HairFast's latent modulation stacks of ``RotateModel``,
+    ``ClipBlendingModel`` and ``PostProcessModel`` on them."""
     if segmentation:
         for ref_name, ours in _SEGMENTATION.items():
             _register(ref_name, ours)
@@ -225,7 +240,11 @@ def install(generator: bool = True, encoders: bool = True, postprocess: bool = T
         for ref_name, ours in _ENCODERS.items():
             _register(ref_name, ours)
     if postprocess:
+        _options["postprocess"] = True
         _post_import.update(_POSTPROCESS)
+    if modulation:
+        _options["modulation"] = True
+        _post_import.add(_MODULATION_MODULE)
     if glue:
         _post_import.update(_GLUE_ATTRS)
     if segmentation and fuse_face_parsing:
@@ -266,6 +285,10 @@ def uninstall() -> None:
     for module in _patched_parsing:
         importlib.import_module("hairfastgan_b200.parsing_fast").unpatch_parsing_module(module)
     _patched_parsing.clear()
+    for module in _patched_modulation:
+        importlib.import_module("hairfastgan_b200.modulation").unpatch_encoders_module(module)
+    _patched_modulation.clear()
+    _options.update(postprocess=False, modulation=False)
     for (module, name), ref in _sean_saved.items():
         setattr(module, name, ref)
     _sean_saved.clear()

@@ -443,6 +443,54 @@ size_t hf_shape_layer_norm_workspace_bytes(long long n);
 int hf_shape_logits_argmax(const void* hair16, const void* face16, const float* table, const float* bias,
                            long long* labels, int res, int dtype, void* stream);
 
+/* ---- HairFast's latent modulation stacks (models/Encoders.py:13-137) ---- */
+/* One call covers `stacks` stacks of 5 ModulationModule(layers, inp, middle) for `batch` samples: rows = batch *
+ * layers.  Branch j of a stack (0..9) is module j / 2's gamma_function (j even) or beta_function (j odd).  Every call
+ * taking a descriptor returns HF_ERR_INVALID ("<call>: bad dtype N") for a dtype other than HF_BF16 / HF_F16 before
+ * it checks its other arguments.  Supported: 1 <= layers <= 24, inp = 512 * n with n * stacks <= 3, middle a multiple
+ * of 256 up to 1024, stacks 1 or 2. */
+typedef struct {
+  int layers; /* L, rows per sample */
+  int inp;    /* embedding width */
+  int middle; /* gamma / beta hidden width */
+  int stacks; /* 1, or 2 for PostProcessModel's to_latent_1 / to_latent_2 */
+  int dtype;  /* HF_BF16 / HF_F16: operands, hidden rows */
+} hf_mod_desc;
+/* fp32 rows [batch][layers][512] with unit column stride; strides in elements (0 broadcasts). */
+typedef struct {
+  const float* ptr;
+  long long batch_stride;
+  long long row_stride;
+} hf_mod_rows;
+
+/* Scratch of hf_mod_gemm, hf_mod_hidden and hf_mod_chain for one call's descriptor and batch (needs a device). */
+size_t hf_mod_workspace_bytes(const hf_mod_desc* d, int batch);
+/* The split-K plan of style layer 1 or 2 on a device with `sms` SMs (needs no device): out[5] = {row tile, K splits,
+ * 64-wide K tiles, output tiles, row tiles}. */
+int hf_mod_gemm_plan(const hf_mod_desc* d, int batch, int layer, int sms, int* out);
+/* The 16-bit embedding e16 [stacks][rows][inp]: stack s's columns 512 j .. 512 j + 511 are src[s * inp / 512 + j]. */
+int hf_mod_embed16(const hf_mod_desc* d, int batch, const hf_mod_rows* src, void* e16, void* stream);
+/* Grouped split-K GEMM of style layer 1 or 2, y32 = x16 w16^T + bias, partials added in split order:
+ *   layer 1: stacks groups, w16 [stacks][10 middle][inp], x16 = e16 [stacks][rows][inp], bias [stacks][10 middle],
+ *            y32 [stacks][rows][10 middle];
+ *   layer 2: 10 stacks groups, w16 [10 stacks][512][middle], x16 = h16 [rows][10 stacks middle] (group g reads
+ *            columns g middle ..), bias [10 stacks][512], y32 = gamma / beta [10 stacks][rows][512].
+ * bias may be NULL. */
+int hf_mod_gemm(const hf_mod_desc* d, int batch, int layer, const void* w16, const void* x16, const float* bias,
+                float* y32, float* workspace, void* stream);
+/* Style layer 1 with the rest of Linear -> LayerNorm([middle]) -> LeakyReLU(0.01) fused into its reduction:
+ * h16[p][(s 10 + j) middle + n] for branch j of stack s; bias [stacks][10 middle], ln_w / ln_b [stacks][10][middle]
+ * (biased variance, eps 1e-5). */
+int hf_mod_hidden(const hf_mod_desc* d, int batch, const void* w16, const void* e16, const float* bias,
+                  const float* ln_w, const float* ln_b, void* h16, float* workspace, void* stream);
+/* The fc chain on thread-block clusters of 8 CTAs per (stack, sample): PixelNorm over the layers of x0[s], then per
+ * module fc (fc_w16 [stacks][5][512][512], fc_b [stacks][5][512]), LayerNorm over the whole [layers, 512] sample,
+ * x (1 + gamma) + beta (gb from hf_mod_gemm layer 2) and LeakyReLU(0.01) except after the last module.
+ * out [batch][layers][512] = base + 0.1 dt for one stack, base + 0.1 (dt_0 + dt_1) for two.  One kernel launch; with
+ * two stacks it is preceded by a cudaMemsetAsync of the completion counters in the workspace. */
+int hf_mod_chain(const hf_mod_desc* d, int batch, const void* fc_w16, const float* fc_b, const float* gb,
+                 const hf_mod_rows* x0, const hf_mod_rows* base, float* out, float* workspace, void* stream);
+
 /* Number of kernels the last hf_generator_forward / hf_conv_forward of this thread launched. */
 int hf_last_launch_count(void);
 /* Number of kernels every hf_* call of this thread has launched since the library was loaded. */
