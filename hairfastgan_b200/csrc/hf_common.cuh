@@ -49,6 +49,9 @@ int encode_tmap(CUtensorMap* map, int dtype, int rank, void* gaddr, const uint64
   } while (0)
 
 inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
+// every pointer 16-byte aligned (a null pointer counts as aligned): the precondition of uint4 / float4 accesses
+template <class... P>
+inline bool aligned16(P... p) { return (((uintptr_t)p | ... | (uintptr_t)0) & 15) == 0; }
 // grid of a 256-thread grid-stride loop over n items: at most 16 CTAs per SM
 inline int grid_for(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, (int64_t)num_sms() * 16); }
 

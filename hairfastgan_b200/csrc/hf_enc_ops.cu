@@ -220,6 +220,7 @@ static int channel_reduce_splits(int B, int HW, int C) {
 static int channel_partial(const void* x16, const float* center, float* ws, int B, int HW, int C, int dtype,
                            cudaStream_t st, int* splits) {
   HF_REQUIRE(x16 && ws && C % 8 == 0 && B > 0 && HW > 0, "channel_partial: bad arguments");
+  HF_REQUIRE(aligned16(x16), "channel_partial: the 16-bit tensor must be 16-byte aligned");
   const int S = channel_reduce_splits(B, HW, C), chunk = cdiv(HW, S);
   dim3 grid(cdiv(C, 64), B, S);
   const uint16_t* x = (const uint16_t*)x16;
@@ -566,6 +567,7 @@ int hf_instance_norm_lrelu_nhwc16(const void* x16, void* y16, void* workspace, i
     cudaStream_t st = (cudaStream_t)stream;
     HF_REQUIRE(x16 && y16 && ws, "instance_norm: null pointer");
     HF_REQUIRE(B > 0 && HW > 0 && C > 0 && C % 8 == 0, "instance_norm: bad shape B=%d HW=%d C=%d (C %% 8)", B, HW, C);
+    HF_REQUIRE(aligned16(x16, y16), "instance_norm: 16-bit tensors must be 16-byte aligned");
     const int64_t total8 = (int64_t)B * HW * C / 8;
     HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch",
                (long long)total8);
@@ -634,6 +636,7 @@ int hf_scale_add_nhwc16(const void* res16, const float* se, const void* shortcut
     cudaStream_t st = (cudaStream_t)stream;
     HF_REQUIRE(res16 && (y16 || y16b), "scale_add: null pointer");
     HF_REQUIRE(C % 2 == 0 && (sc_stride == 1 || sc_stride == 2), "scale_add: bad C / stride");
+    HF_REQUIRE(aligned16(res16, shortcut16, y16, y16b, se), "scale_add: 16-bit tensors and se must be 16-byte aligned");
     if (C % 8 == 0) {
       const int64_t total8 = (int64_t)B * H * W * C / 8;
       HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
@@ -662,6 +665,7 @@ int hf_upsample_add_nhwc16(const void* x16, const void* y16, void* out16, int B,
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     HF_REQUIRE(x16 && y16 && out16 && C % 2 == 0, "upsample_add: bad arguments");
+    HF_REQUIRE(aligned16(x16, y16, out16), "upsample_add: 16-bit tensors must be 16-byte aligned");
     if (C % 8 == 0) {
       const int64_t total8 = (int64_t)B * H * W * C / 8;
       HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
@@ -688,6 +692,7 @@ int hf_adaptive_avgpool_nhwc16(const void* x16, float* y, int B, int H, int W, i
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     HF_REQUIRE(x16 && y && oh > 0 && ow > 0, "adaptive_avgpool: bad arguments");
+    HF_REQUIRE(aligned16(x16), "adaptive_avgpool: the 16-bit tensor must be 16-byte aligned");
     if (C % 8 == 0 && (int64_t)oh * ow <= 65535 && B <= 65535) {
       dim3 grid(cdiv(C, 64), oh * ow, B);
       adaptive_avgpool_vec8_kernel<dt><<<grid, 256, 0, st>>>((const uint16_t*)x16, y, H, W, C, oh, ow);

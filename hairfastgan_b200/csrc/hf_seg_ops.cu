@@ -9,7 +9,8 @@
 namespace hf {
 
 // ------------------------------------------------------------------------------------------------
-// nn.MaxPool2d(kernel_size=3, stride=2, padding=1) (resnet.py:62,71) on NHWC 16-bit; padding never wins the max.
+// nn.MaxPool2d(kernel_size=3, stride=2, padding=1) (resnet.py:62,71) on NHWC 16-bit.  The padding is skipped, not
+// read: the running max starts at -inf, so a window of -inf (or of bf16's lowest finite value, -3.39e38) returns it.
 // ------------------------------------------------------------------------------------------------
 template <int DT>
 __global__ void __launch_bounds__(256) maxpool3x3s2_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y,
@@ -23,7 +24,7 @@ __global__ void __launch_bounds__(256) maxpool3x3s2_kernel(const uint16_t* __res
     const int b = (int)(t / Ho);
     float m[8];
 #pragma unroll
-    for (int k = 0; k < 8; ++k) m[k] = -3.0e38f;
+    for (int k = 0; k < 8; ++k) m[k] = -INFINITY;
 #pragma unroll
     for (int dy = -1; dy <= 1; ++dy) {
       const int yy = 2 * oy + dy;
@@ -494,6 +495,7 @@ int hf_maxpool3x3s2_nhwc16(const void* x16, void* y16, int B, int H, int W, int 
     int rc = ensure_device_current();
     if (rc) return rc;
     HF_REQUIRE(x16 && y16 && C % 8 == 0 && B > 0 && H > 0 && W > 0, "maxpool: bad arguments");
+    HF_REQUIRE(aligned16(x16, y16), "maxpool: 16-bit tensors must be 16-byte aligned");
     const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
     const int64_t total8 = (int64_t)B * Ho * Wo * C / 8;
     HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
@@ -531,6 +533,7 @@ int hf_gate_add_up_nhwc16(const void* x16, const float* gate, const float* addve
     if (rc) return rc;
     HF_REQUIRE(x16 && y16 && C % 8 == 0 && (up == 1 || up == 2) && B > 0 && h > 0 && w > 0,
                "gate_add_up: bad arguments");
+    HF_REQUIRE(aligned16(x16, addt16, y16), "gate_add_up: 16-bit tensors must be 16-byte aligned");
     const int64_t total8 = (int64_t)B * h * up * w * up * C / 8;
     HF_REQUIRE(total8 < (int64_t)2000000000, "tensor too large for one launch (%lld work items): split the batch", (long long)total8);
     gate_add_up_kernel<dt><<<grid_for(total8), 256, 0, (cudaStream_t)stream>>>(

@@ -178,8 +178,16 @@ def se_gate(x16: torch.Tensor, fc1_weight: torch.Tensor, fc2_weight: torch.Tenso
 
 def scale_add(res16, se=None, shortcut16=None, shortcut_stride: int = 1, y16b_affine=None, want_y16: bool = True,
               dtype: Optional[int] = None):
+    """res16 * se[b,c] + shortcut16[:, ::s, ::s] (s = shortcut_stride): the shortcut must be [B, H*s, W*s, C].  The
+    MaxPool2d(1, 2) shortcut of an odd (2H-1) x (2W-1) input also subsamples to H x W, but the kernel indexes the
+    shortcut with the pitch of 2H x 2W, so that shape is rejected here rather than read out of bounds."""
     dt = default_dtype() if dtype is None else dtype
     b, h, w, c = res16.shape
+    if shortcut16 is not None:
+        want = (b, h * shortcut_stride, w * shortcut_stride, c)
+        if tuple(shortcut16.shape) != want:
+            raise ValueError(f"scale_add: shortcut of shape {list(shortcut16.shape)}, expected {list(want)} "
+                             f"for stride {shortcut_stride}")
     y = torch.empty_like(res16) if want_y16 else None
     yb, s2, b2 = None, None, None
     if y16b_affine is not None:

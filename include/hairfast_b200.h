@@ -256,14 +256,16 @@ int hf_nhwc16_to_nchw(const void* x16, float* y, int batch, int channels, int he
 size_t hf_instance_norm_workspace_bytes(int batch, int hw, int channels);
 /* nn.InstanceNorm2d(affine=False, track_running_stats=False) + nn.LeakyReLU(slope) on x16 [B,HW,C] 16-bit NHWC -> y16
  * (may alias x16): per-(b, c) mean, then the biased variance of the centred values (two passes, eps 1e-5), fp32
- * statistics in a fixed summation order (the reduction of hf_channel_mean_nhwc16).  channels % 8 == 0. */
+ * statistics in a fixed summation order (the reduction of hf_channel_mean_nhwc16).  channels % 8 == 0; x16 and y16
+ * 16-byte aligned. */
 int hf_instance_norm_lrelu_nhwc16(const void* x16, void* y16, void* workspace, int batch, int hw, int channels,
                                   float slope, int dtype, void* stream);
 /* nn.ReflectionPad2d(1): x16 [B,H,W,C] -> y16 [B,H+2,W+2,C] 16-bit NHWC.  H, W >= 2, channels % 8 == 0. */
 int hf_reflect_pad1_nhwc16(const void* x16, void* y16, int batch, int height, int width, int channels, int dtype,
                            void* stream);
 
-/* Scratch (bytes) for the two-stage deterministic channel reduction below. */
+/* The five calls below move 16 bytes at a time: their 16-bit tensors, and se, must be 16-byte aligned (else
+ * HF_ERR_INVALID, nothing launched).  Scratch (bytes) for the two-stage deterministic channel reduction below. */
 size_t hf_channel_reduce_workspace_bytes(int batch, int hw, int channels);
 /* SEModule.avg_pool (helpers.py:60): mean over H*W -> [B,C] fp32.  channels % 8 == 0. */
 int hf_channel_mean_nhwc16(const void* x16, float* mean, void* workspace, int batch, int hw, int channels, int dtype,
@@ -299,18 +301,19 @@ int hf_stem3x3_nhwc16(const float* x, const void* wpacked, const float* shift, c
 int hf_stem7x7s2_nhwc16(const float* x, const void* wpacked, const float* shift, void* y16, int batch, int height,
                         int width, int dtype, void* stream);
 
-/* nn.MaxPool2d(3, 2, 1) (resnet.py:62,71) on 16-bit NHWC; output (H-1)/2+1 x (W-1)/2+1 */
+/* nn.MaxPool2d(3, 2, 1) (resnet.py:62,71) on 16-bit NHWC; output (H-1)/2+1 x (W-1)/2+1; both 16-byte aligned */
 int hf_maxpool3x3s2_nhwc16(const void* x16, void* y16, int batch, int height, int width, int channels, int dtype,
                            void* stream);
 /* 1x1 conv of the globally pooled feature + folded BatchNorm + activation (act: 0 none, 1 ReLU, 2 sigmoid):
  * out[b,o] = act((sum_c weight[o,c] * mean_hw(x)[b,c]) * scale[o] + shift[o]); scale / shift may be NULL.
  * AttentionRefinementModule attention (model.py:82-86), ContextPath.conv_avg (model.py:114-115).
- * workspace: hf_channel_reduce_workspace_bytes(batch, hw, channels). */
+ * workspace: hf_channel_reduce_workspace_bytes(batch, hw, channels); x16 16-byte aligned. */
 int hf_pooled_fc_nhwc16(const void* x16, const float* weight, const float* scale, const float* shift, int act,
                         float* out, void* workspace, int batch, int hw, int channels, int cout, int dtype,
                         void* stream);
 /* ContextPath merge (model.py:116-128): y[b,Y,X,c] = x[b,Y/up,X/up,c]*gate[b,c] + addvec[b,c] + addt[b,Y/up,X/up,c];
- * up = 1 or 2 (F.interpolate nearest); gate / addvec / addt16 may be NULL; height, width = input size. */
+ * up = 1 or 2 (F.interpolate nearest); gate / addvec / addt16 may be NULL; height, width = input size; the 16-bit
+ * tensors 16-byte aligned. */
 int hf_gate_add_up_nhwc16(const void* x16, const float* gate, const float* addvec, const void* addt16, void* y16,
                           int batch, int height, int width, int channels, int up, int dtype, void* stream);
 /* F.interpolate(bilinear, align_corners=True) (model.py:239-241) of the first `channels` of `in_channels` planes:

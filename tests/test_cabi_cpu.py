@@ -58,6 +58,56 @@ def test_argument_validation_without_device(lib):
     assert h.hf_upfirdn2d_f32(None, None, None, 0, 4, 4, 4, 4, 1, 1, 1, 1, 0, 0, 0, 0, None) == 0   # empty input
 
 
+no_device_only = pytest.mark.skipif(torch.cuda.is_available(),
+                                    reason="hands the library fake pointers: only where no CUDA device could run them")
+
+
+@no_device_only
+@pytest.mark.parametrize("dt", ["HF_BF16", "HF_F16"])
+def test_unaligned_16bit_tensors_rejected_without_device(lib, dt):
+    """Every SIMT entry point whose kernel moves 16 bytes at a time rejects a pointer that is only 8-byte aligned
+    (0x...8), before any launch, on either path (vec8 or scalar)."""
+    h, d = lib.lib(), getattr(lib, dt)
+    A, B_, C_, D_, U = 0x10000, 0x20000, 0x30000, 0x40000, 0x50008       # U: 8-byte aligned, not 16
+    part = b"channel_partial: the 16-bit tensor must be 16-byte aligned"
+    cases = [
+        (h.hf_channel_mean_nhwc16, (U, A, B_, 1, 4, 8, d, None), part),
+        (h.hf_se_gate_nhwc16, (U, A, B_, C_, D_, 1, 4, 8, 2, d, None), part),
+        (h.hf_pooled_fc_nhwc16, (U, A, None, None, 0, B_, C_, 1, 4, 8, 3, d, None), part),
+        (h.hf_instance_norm_lrelu_nhwc16, (U, A, B_, 1, 4, 8, 0.2, d, None), b"instance_norm: 16-bit tensors"),
+        (h.hf_instance_norm_lrelu_nhwc16, (A, U, B_, 1, 4, 8, 0.2, d, None), b"instance_norm: 16-bit tensors"),
+        (h.hf_scale_add_nhwc16, (U, None, None, 1, None, None, A, None, 1, 2, 2, 8, d, None), b"scale_add: 16-bit"),
+        (h.hf_scale_add_nhwc16, (A, U, None, 1, None, None, B_, None, 1, 2, 2, 8, d, None), b"scale_add: 16-bit"),
+        (h.hf_scale_add_nhwc16, (A, None, U, 2, None, None, B_, None, 1, 2, 2, 8, d, None), b"scale_add: 16-bit"),
+        (h.hf_scale_add_nhwc16, (A, None, None, 1, B_, C_, None, U, 1, 2, 2, 8, d, None), b"scale_add: 16-bit"),
+        (h.hf_scale_add_nhwc16, (U, None, None, 1, None, None, A, None, 1, 2, 2, 6, d, None), b"scale_add: 16-bit"),
+        (h.hf_upsample_add_nhwc16, (U, A, B_, 1, 2, 2, 4, 4, 8, d, None), b"upsample_add: 16-bit"),
+        (h.hf_upsample_add_nhwc16, (A, B_, U, 1, 2, 2, 4, 4, 6, d, None), b"upsample_add: 16-bit"),
+        (h.hf_adaptive_avgpool_nhwc16, (U, A, 1, 4, 4, 8, 2, 2, d, None), b"adaptive_avgpool: the 16-bit tensor"),
+        (h.hf_adaptive_avgpool_nhwc16, (U, A, 1, 4, 4, 6, 2, 2, d, None), b"adaptive_avgpool: the 16-bit tensor"),
+        (h.hf_maxpool3x3s2_nhwc16, (U, A, 1, 4, 4, 8, d, None), b"maxpool: 16-bit tensors"),
+        (h.hf_maxpool3x3s2_nhwc16, (A, U, 1, 4, 4, 8, d, None), b"maxpool: 16-bit tensors"),
+        (h.hf_gate_add_up_nhwc16, (U, None, None, None, A, 1, 2, 2, 8, 2, d, None), b"gate_add_up: 16-bit"),
+        (h.hf_gate_add_up_nhwc16, (A, None, None, U, B_, 1, 2, 2, 8, 1, d, None), b"gate_add_up: 16-bit"),
+        (h.hf_gate_add_up_nhwc16, (A, B_, C_, None, U, 1, 2, 2, 8, 2, d, None), b"gate_add_up: 16-bit"),
+    ]
+    for fn, args, msg in cases:
+        assert fn(*args) == -1, (fn.__name__, args)                   # HF_ERR_INVALID
+        assert h.hf_last_error().startswith(msg), (fn.__name__, args, h.hf_last_error())
+
+
+@no_device_only
+def test_scale_add_rejects_a_shortcut_of_the_wrong_shape():
+    """MaxPool2d(1, 2) of an odd (2H-1) x (2W-1) map also has H x W pixels, but the kernel reads its stride-2
+    shortcut as [B, 2H, 2W, C]: the wrapper refuses any other shape before the library sees it."""
+    import hairfastgan_b200.nn16 as N
+    res = torch.zeros(2, 4, 5, 8, dtype=torch.float16)
+    for sc, stride in (((2, 7, 9, 8), 2), ((2, 8, 9, 8), 2), ((2, 8, 10, 8), 1), ((1, 8, 10, 8), 2),
+                       ((2, 8, 10, 16), 2)):
+        with pytest.raises(ValueError, match="scale_add: shortcut of shape"):
+            N.scale_add(res, shortcut16=torch.zeros(sc, dtype=torch.float16), shortcut_stride=stride)
+
+
 def test_every_dtype_argument_is_checked_first(lib):
     """Every call with an `int dtype` parameter rejects a value other than HF_BF16 / HF_F16 before its other
     argument checks: with every other argument zero / NULL the error names the dtype."""
