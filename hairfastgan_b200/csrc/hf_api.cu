@@ -229,6 +229,8 @@ static int conv_forward_impl(const hf_conv_desc* d, const void* packed, const hf
                              int time_iters, float* avg_ms) {
   int rc = check_desc(d);
   if (rc) return rc;
+  HF_REQUIRE(!io || aligned16(io->style, io->mod_weight),
+             "hf_conv_forward: style and mod_weight must be 16-byte aligned");      // float4 loads of the affine
   if ((rc = ensure_device_current())) return rc;
   reset_launch_count();
   HF_REQUIRE(packed && io && io->x && io->style && io->mod_weight && io->mod_bias && io->y && io->workspace,
@@ -336,6 +338,8 @@ int hf_torgb_forward(const float* x, const float* style, int64_t style_stride, i
                      const float* conv_weight, const float* mod_weight, const float* mod_bias, const float* bias,
                      const float* up_kernel, const float* skip, float* y, int batch, int cin, int height, int width,
                      void* workspace, void* stream) {
+  // the style affine reads style and mod_weight rows with float4 loads: checked before anything touches a device
+  HF_REQUIRE(aligned16(style, mod_weight), "hf_torgb_forward: style and mod_weight must be 16-byte aligned");
   int rc = ensure_device_current();
   if (rc) return rc;
   reset_launch_count();

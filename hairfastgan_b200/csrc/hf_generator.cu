@@ -227,6 +227,8 @@ int hf_generator_forward(const hf_gen_config* cfg, const void* packed, const hf_
   GenLayout L;
   int rc = make_layout(cfg, &L);
   if (rc) return rc;
+  // the style affine reads the latent rows with float4 loads: checked before anything touches a device
+  HF_REQUIRE(!io || aligned16(io->latent), "hf_generator_forward: latent must be 16-byte aligned");
   if ((rc = ensure_device_current())) return rc;
   reset_launch_count();
   HF_REQUIRE(packed && io && workspace, "hf_generator_forward: null pointer");
@@ -320,6 +322,9 @@ int hf_generator_forward(const hf_gen_config* cfg, const void* packed, const hf_
     prof_begin(st);
     int r = launch_conv(cl, st, &pl);
     prof_end(st, "conv", i, s.cin, s.cout, s.res_in, s.up, pl.n_tile, pl.halo);
+    // the early exit's out_feature and return_features ask for the same activation; the epilogue stores one of them
+    if (r == HF_OK && out_nchw && cl.out_nchw != out_nchw)
+      r = launch_scale_copy(cl.out_nchw, out_nchw, (int64_t)B * s.cout * s.res_out * s.res_out, 1.f, st);
     if (num_nt) *num_nt = pl.num_n_tiles;
     return r;
   };

@@ -86,7 +86,8 @@ typedef struct {
   int batch, height, width;  /* input spatial size */
   const float* x;            /* [B,cin,H,W] fp32 NCHW; batch_stride_x = 0 broadcasts one sample */
   int x_batch_broadcast;
-  const float* style;        /* [B, style_dim] latent rows for this layer (row stride style_stride) */
+  const float* style;        /* [B, style_dim] latent rows for this layer (row stride style_stride); style and
+                                mod_weight 16-byte aligned (else HF_ERR_INVALID, nothing launched) */
   int style_dim;
   int64_t style_stride;
   const float* mod_weight;   /* conv.modulation.weight [cin, style_dim] */
@@ -123,7 +124,8 @@ int hf_conv_time_kernel(const hf_conv_desc* d, const void* packed, const hf_conv
                         float* avg_ms /* host */, void* stream);
 
 /* Replaces ToRGB.forward (model.py:356-365): modulated 1x1 conv without demodulation + bias +
- * Upsample(skip) (model.py:35-53).  x [B,cin,H,W], skip [B,3,H/2,W/2] or NULL, y [B,3,H,W]; fp32. */
+ * Upsample(skip) (model.py:35-53).  x [B,cin,H,W], skip [B,3,H/2,W/2] or NULL, y [B,3,H,W]; fp32.
+ * style and mod_weight must be 16-byte aligned (else HF_ERR_INVALID, nothing launched). */
 int hf_torgb_forward(const float* x, const float* style, int64_t style_stride, int style_dim,
                      const float* conv_weight /* [1,3,cin,1,1] */, const float* mod_weight,
                      const float* mod_bias, const float* bias /* [1,3,1,1] */,
@@ -166,7 +168,8 @@ int hf_generator_pack(const hf_gen_config* cfg, const hf_gen_weights* w, void* p
 
 typedef struct {
   int batch;
-  const float* latent;   /* [B, n_latent, style_dim] fp32 (input_is_latent=True, model.py:521-522) */
+  const float* latent;   /* [B, n_latent, style_dim] fp32 (input_is_latent=True, model.py:521-522), 16-byte aligned
+                            (else HF_ERR_INVALID, nothing launched) */
   const float* noise[HF_MAX_STYLED]; /* per styled conv: [noise_batch,1,R,R] fp32 (explicit; the host
                                         draws random noise in reference order, model.py:288-291) */
   int noise_batch[HF_MAX_STYLED];    /* 1 = shared across the batch (registered buffers), or B */
@@ -180,7 +183,7 @@ typedef struct {
    * index i (i >= 1; [B,Cin_i,R,R] fp32 NCHW or NULL).  Only alpha == 1 (what HairFast runs:
    * min(1, 1e-4 * n_iter) with n_iter = 1e5, trainer.py:358-359) is implemented.
    * return_features: features_out[0] = ConstantInput output, features_out[i+1] = output of styled conv i
-   * ([B,Cout_i,R,R] fp32 NCHW each; NULL entries are skipped). */
+   * ([B,Cout_i,R,R] fp32 NCHW each; NULL entries are skipped; an early exit still fills out_feature as well). */
   const float* feature_in[HF_MAX_STYLED];
   float feature_alpha;
   float* features_out[HF_MAX_STYLED + 1];

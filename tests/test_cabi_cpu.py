@@ -97,6 +97,31 @@ def test_unaligned_16bit_tensors_rejected_without_device(lib, dt):
 
 
 @no_device_only
+def test_unaligned_style_rows_rejected_without_device(lib):
+    """The style affine reads latent rows and modulation weights with float4 loads: hf_torgb_forward,
+    hf_conv_forward and hf_generator_forward reject a pointer that is only 4-byte aligned (0x...4), before any
+    launch."""
+    h = lib.lib()
+    A, B_, U = 0x10000, 0x20000, 0x50004                                # U: 4-byte aligned, not 16
+    msg = b"hf_torgb_forward: style and mod_weight must be 16-byte aligned"
+    for style, mw in ((U, A), (A, U)):
+        assert h.hf_torgb_forward(A, style, 512, 512, A, mw, B_, B_, None, None, A, 1, 64, 4, 4, A, None) == -1
+        assert h.hf_last_error() == msg, h.hf_last_error()
+    d = lib.hf_conv_desc(64, 64, 3, 0, lib.HF_BF16)
+    for style, mw in ((U, A), (A, U)):
+        io = lib.hf_conv_io()
+        io.batch, io.height, io.width, io.x, io.style, io.style_dim, io.style_stride = 1, 4, 4, A, style, 512, 512
+        io.mod_weight, io.mod_bias, io.y, io.workspace = mw, B_, A, A
+        assert h.hf_conv_forward(C.byref(d), A, C.byref(io), None) == -1
+        assert h.hf_last_error() == b"hf_conv_forward: style and mod_weight must be 16-byte aligned", h.hf_last_error()
+    cfg = lib.hf_gen_config(64, 512, 2, lib.HF_BF16)
+    io = lib.hf_gen_io()
+    io.batch, io.latent, io.out_rgb = 1, U, A
+    assert h.hf_generator_forward(C.byref(cfg), A, C.byref(io), A, None, None) == -1
+    assert h.hf_last_error() == b"hf_generator_forward: latent must be 16-byte aligned", h.hf_last_error()
+
+
+@no_device_only
 def test_scale_add_rejects_a_shortcut_of_the_wrong_shape():
     """MaxPool2d(1, 2) of an odd (2H-1) x (2W-1) map also has H x W pixels, but the kernel reads its stride-2
     shortcut as [B, 2H, 2W, C]: the wrapper refuses any other shape before the library sees it."""
