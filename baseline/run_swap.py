@@ -1,7 +1,8 @@
 """One process = one arm of the full `HairFast.swap()` comparison (BASELINE configs[2], SURVEY 8d config 3).
 
     python baseline/run_swap.py --mode reference|overlay|overlay_fast|overlay_sean|overlay_sean_full|overlay_all|
-                                       overlay_modulation --work DIR --out result.pt [--reps N]
+                                       overlay_modulation|reference_align|overlay_align --work DIR --out result.pt
+                                [--reps N]
 
 * reference     the unmodified reference (oracle/_ref): cuDNN grouped convolutions + its two JIT kernels, fp32/TF32
 * overlay       the same checkout with hairfastgan_b200.install() active (this package's modules under its names)
@@ -11,6 +12,10 @@
 * overlay_all        overlay_sean_full + install(shape_adaptor=True): CtrlHair's shape adaptor on it too
 * overlay_modulation overlay_all + install(modulation=True): HairFast's Rotate / Blending / PostProcess latent
                      modulation stacks on it too
+* reference_align    the stock reference called as swap(face, shape, color, align=True): dlib inside
+                     utils.shape_predictor is replaced by oracle/align_oracle.FakeDlib, whose predictor returns the
+                     landmarks of tests/golden/align.npz's "crop", "pad" and "tilted" cases for the three images
+* overlay_align      the same aligned swap under overlay_all + install(face_align=True)
 
 Three synthetic images `torch.rand(3,1024,1024)` (seeds 0,1,2) are passed as tensors (hair_swap.py:63-105), synthetic
 checkpoints come from baseline/synth_checkpoints.py, `swap(..., seed=3407)` is the default seed (utils/seed.py:22-28).
@@ -32,10 +37,28 @@ sys.path.insert(0, os.path.dirname(HERE))
 from baseline import refenv, synth_checkpoints  # noqa: E402
 
 
+def _fake_landmarks():
+    """Aligned-swap modes: a fake dlib in utils.shape_predictor whose predictor cycles through three golden landmark
+    sets, and a placeholder predictor file so align_face (shape_predictor.py:85-94) loads instead of downloading."""
+    import numpy as np
+    import PIL.Image
+    import utils.shape_predictor as sp
+    from oracle.align_oracle import FakeDlib
+    gold = np.load(os.path.join(os.path.dirname(HERE), "tests", "golden", "align.npz"))
+    sp.dlib = FakeDlib([gold[f"{n}_lm"] for n in ("crop", "pad", "tilted")])
+    if not hasattr(PIL.Image, "ANTIALIAS"):          # the shrink branch's name for LANCZOS (Pillow < 10)
+        PIL.Image.ANTIALIAS = PIL.Image.LANCZOS
+    path = os.path.join("pretrained_models", "ShapeAdaptor", "shape_predictor_68_face_landmarks.dat")
+    if not os.path.isfile(path):
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        with open(path, "wb") as f:
+            f.write(b"placeholder: the fake dlib does not read it\n")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--mode", choices=["reference", "overlay", "overlay_fast", "overlay_sean", "overlay_sean_full",
-                                       "overlay_all", "overlay_modulation"],
+                                       "overlay_all", "overlay_modulation", "reference_align", "overlay_align"],
                     required=True)
     ap.add_argument("--work", default="/tmp/hairfast_work")
     ap.add_argument("--out", default=None)
@@ -54,12 +77,17 @@ def main():
     sean = {"overlay_sean": {"sean": True}, "overlay_sean_full": {"sean": True, "sean_encode": True},
             "overlay_all": {"sean": True, "sean_encode": True, "shape_adaptor": True},
             "overlay_modulation": {"sean": True, "sean_encode": True, "shape_adaptor": True,
-                                   "modulation": True}}.get(a.mode, {})
-    refenv.activate(overlay=a.mode != "reference", skip_fse_reconstruction=a.mode == "overlay_fast", workdir=work,
-                    **sean)
+                                   "modulation": True},
+            "overlay_align": {"sean": True, "sean_encode": True, "shape_adaptor": True, "face_align": True}
+            }.get(a.mode, {})
+    align = a.mode in ("reference_align", "overlay_align")
+    refenv.activate(overlay=a.mode not in ("reference", "reference_align"),
+                    skip_fse_reconstruction=a.mode == "overlay_fast", workdir=work, **sean)
     import torch
     assert torch.cuda.is_available(), "run_swap.py needs a GPU (tools/dryrun_swap_cpu.py is the CPU dry run)"
     from hair_swap import HairFast, get_parser      # the reference's own hair_swap.py
+    if align:
+        _fake_landmarks()
 
     t0 = time.time()
     hair_fast = HairFast(get_parser().parse_args([]))
@@ -159,7 +187,9 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         w0 = time.time()
         e0.record()
-        final = hair_fast.swap(*imgs, **kw)
+        final = hair_fast.swap(*imgs, align=True, **kw) if align else hair_fast.swap(*imgs, **kw)
+        if align:
+            final, *aligned = final
         e1.record()
         torch.cuda.synchronize()
         wall = (time.time() - w0) * 1e3
@@ -178,6 +208,8 @@ def main():
             print("TRACE " + json.dumps(line), file=sys.stderr, flush=True)
         if rep >= a.warmup:
             finals.append(final.detach().float().cpu())
+            if align:
+                captured_aligned = [t.detach().cpu() for t in aligned]
             timings.append({"wall_ms": wall, "gpu_ms": e0.elapsed_time(e1), "hot_path_ms": hot_ms,
                             "out_of_scope_ms": e0.elapsed_time(e1) - hot_ms, "per_module_ms": per,
                             "hot_calls": len(spans)})
@@ -196,7 +228,10 @@ def main():
                "cuda_peak_allocated_gb": round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)}
     print(json.dumps(summary))
     if a.out:
-        torch.save({"finals": finals, "embed": dict(captured), "summary": summary}, a.out)
+        res = {"finals": finals, "embed": dict(captured), "summary": summary}
+        if align:
+            res["aligned"] = captured_aligned
+        torch.save(res, a.out)
 
 
 if __name__ == "__main__":

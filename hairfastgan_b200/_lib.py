@@ -176,6 +176,20 @@ SYMBOLS = {
     "hf_mod_hidden": (C.c_int, [C.POINTER(hf_mod_desc), C.c_int] + [C.c_void_p] * 8),
     "hf_mod_chain": (C.c_int, [C.POINTER(hf_mod_desc), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                C.POINTER(hf_mod_rows), C.POINTER(hf_mod_rows), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "hf_align_lanczos_taps": (C.c_int, [C.c_int, C.c_int]),
+    "hf_align_lanczos_coeffs": (C.c_int, [C.c_int, C.c_int, C.c_void_p]),
+    "hf_align_resample_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "hf_align_resample_u8": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "hf_align_pad_blend_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "hf_align_pad_blend_u8": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.c_void_p,
+                                        C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "hf_align_gaussian_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                        C.c_void_p]),
+    "hf_align_median_workspace_bytes": (C.c_size_t, []),
+    "hf_align_median_f32": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "hf_align_quad_u8": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.c_void_p,
+                                   C.c_int, C.c_int, C.c_void_p]),
     "hf_generator_packed_bytes":(C.c_size_t, [C.POINTER(hf_gen_config)]),
     "hf_generator_workspace_bytes": (C.c_size_t, [C.POINTER(hf_gen_config), C.c_int]),
     "hf_generator_pack": (C.c_int, [C.POINTER(hf_gen_config), C.POINTER(hf_gen_weights), C.c_void_p, C.c_void_p]),

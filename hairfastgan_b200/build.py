@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libhairfast_sm90.so")
 SOURCES = ["hf_api.cu", "hf_ops.cu", "hf_conv_tc.cu", "hf_generator.cu", "hf_enc_ops.cu",
            "hf_seg_ops.cu", "hf_glue_ops.cu", "hf_sean.cu",
-           "hf_shape.cu", "hf_modulation.cu"]
+           "hf_shape.cu", "hf_modulation.cu", "hf_align.cu"]
 HEADERS = ["hf_common.cuh", "hf_kernels.cuh", "hf_splitk_gemm.cuh", os.path.join("..", "..", "include", "hairfast_b200.h")]
 
 

@@ -41,6 +41,9 @@ After ``install()`` the import statements of the reference resolve to this packa
 * opt-in, ``install(shape_adaptor=True)``: CtrlHair's ``get_hair_face_code`` and ``get_new_shape``
   (models/CtrlHair/shape_branch/solver.py:248-262) are rebound inside that module and ``models.Alignment`` (which
   imports both names, Alignment.py:7)                                               -> ``hairfastgan_b200.shape_adaptor``
+* opt-in, ``install(face_align=True)``: ``align_face`` (utils/shape_predictor.py:80-194) is rebound inside
+  ``utils.shape_predictor`` and ``hair_swap`` (which imports the name, hair_swap.py:19); the landmarks stay on dlib
+                                                                                    -> ``hairfastgan_b200.face_align``
 * opt-in, ``install(modulation=True)``: ``RotateModel.forward``, ``ClipBlendingModel.forward`` and
   ``PostProcessModel.forward`` (models/Encoders.py:66-137) are wrapped inside ``models.Encoders`` after import; the
   classes, their submodules and state-dict keys stay the reference's             -> ``hairfastgan_b200.modulation``
@@ -104,10 +107,12 @@ _patched_parsing = []
 # it), the names chosen by install(), and (module, name) -> the reference function it held
 _SEAN_MODULES = ("models.sean_codes.models.pix2pix_model", "models.Alignment")
 _SHAPE_MODULES = ("models.CtrlHair.shape_branch.solver", "models.Alignment")
+_ALIGN_MODULES = ("utils.shape_predictor", "hair_swap")
 _FUNCTIONS = {"decode_sean": ("hairfastgan_b200.sean", _SEAN_MODULES),
               "encode_sean": ("hairfastgan_b200.sean", _SEAN_MODULES),
               "get_hair_face_code": ("hairfastgan_b200.shape_adaptor", _SHAPE_MODULES),
-              "get_new_shape": ("hairfastgan_b200.shape_adaptor", _SHAPE_MODULES)}
+              "get_new_shape": ("hairfastgan_b200.shape_adaptor", _SHAPE_MODULES),
+              "align_face": ("hairfastgan_b200.face_align", _ALIGN_MODULES)}
 _sean_names = set()
 _sean_saved = {}
 _post_import = set()          # module names the meta-path hook currently patches
@@ -133,7 +138,7 @@ def _patch_sean(module, name: str) -> None:
 
 
 def _patch_postprocess(module) -> None:
-    if module.__name__ in _SEAN_MODULES + _SHAPE_MODULES:
+    if module.__name__ in _SEAN_MODULES + _SHAPE_MODULES + _ALIGN_MODULES:
         for name in sorted(_sean_names):
             if module.__name__ in _FUNCTIONS[name][1]:
                 _patch_sean(module, name)
@@ -216,7 +221,7 @@ def _register(ref_name: str, ours: str) -> None:
 def install(generator: bool = True, encoders: bool = True, postprocess: bool = True, segmentation: bool = True,
             glue: bool = True, skip_fse_reconstruction: bool = False, fuse_face_parsing: bool = True,
             sean: bool = False, sean_encode: bool = False, shape_adaptor: bool = False,
-            modulation: bool = False) -> None:
+            modulation: bool = False, face_align: bool = False) -> None:
     """Register the overlay.  ``generator=False`` swaps only the operator package (L1 boundary) and leaves the
     reference's own ``models/stylegan2/model.py`` classes in place on top of our ops; ``encoders=False`` keeps
     the reference's PyTorch encoders; ``postprocess=False`` keeps its PostProcess conv stack; ``segmentation=False``
@@ -224,7 +229,8 @@ def install(generator: bool = True, encoders: bool = True, postprocess: bool = T
     by default, independent of ``sean``) runs its ``encode_sean`` (the Zencoder) on them; ``shape_adaptor=True`` (off by
     default) runs CtrlHair's shape adaptor (``get_hair_face_code`` / ``get_new_shape``) on them; ``modulation=True``
     (off by default, independent of ``postprocess``) runs HairFast's latent modulation stacks of ``RotateModel``,
-    ``ClipBlendingModel`` and ``PostProcessModel`` on them."""
+    ``ClipBlendingModel`` and ``PostProcessModel`` on them; ``face_align=True`` (off by default) runs the warp of
+    ``align_face`` -- what ``swap(..., align=True)`` and scripts/align_face.py call -- on them."""
     if segmentation:
         for ref_name, ours in _SEGMENTATION.items():
             _register(ref_name, ours)
@@ -260,6 +266,8 @@ def install(generator: bool = True, encoders: bool = True, postprocess: bool = T
         _sean_names.add("encode_sean")
     if shape_adaptor:
         _sean_names.update(("get_hair_face_code", "get_new_shape"))
+    if face_align:
+        _sean_names.add("align_face")
     for name in _sean_names:
         _post_import.update(_FUNCTIONS[name][1])
     if _post_import:

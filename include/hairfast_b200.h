@@ -497,6 +497,38 @@ int hf_mod_hidden(const hf_mod_desc* d, int batch, const void* w16, const void* 
 int hf_mod_chain(const hf_mod_desc* d, int batch, const void* fc_w16, const float* fc_b, const float* gb,
                  const hf_mod_rows* x0, const hf_mod_rows* base, float* out, float* workspace, void* stream);
 
+/* ---- FFHQ face alignment after the landmarks (utils/shape_predictor.py:145-185) ---- */
+/* Images are uint8 RGB, [rows][pitch][3] with `pitch` >= width pixels per row.  Every stage computes what the library
+ * call it replaces computes (DESIGN.md, "Face alignment"). */
+/* Pillow's LANCZOS resampling of one axis from in_size to out_size: taps per output, and the coefficient table
+ * [out_size][taps + 2] int32 (first input, input count, 22-bit fixed-point weights), computed on the host with libm
+ * (needs no device).  taps returns -1 for a size <= 0. */
+int hf_align_lanczos_taps(int in_size, int out_size);
+int hf_align_lanczos_coeffs(int in_size, int out_size, int* table);
+/* Image.resize((Wo, Ho), LANCZOS): horizontal pass (coeff_x = table(W, Wo)) into the workspace, then vertical pass
+ * (coeff_y = table(H, Ho)) into dst [Ho][Wo][3]; a pass whose size does not change is skipped.  Device tables.
+ * workspace hf_align_resample_workspace_bytes(H, W, Ho, Wo) bytes (0: none needed). */
+size_t hf_align_resample_workspace_bytes(int H, int W, int Ho, int Wo);
+int hf_align_resample_u8(const uint8_t* src, int H, int W, int src_pitch, uint8_t* dst, int Ho, int Wo,
+                         const int* coeff_x, const int* coeff_y, uint8_t* workspace, void* stream);
+/* The padding branch (:170-178) on src [H][W]: pad = {left, top, right, bottom} (host, each > 0), weights = the
+ * scipy Gaussian of sigma qsize * 0.02 from its centre outwards, [radius + 1] float64 on the device; dst [H + top +
+ * bottom][W + left + right][3].  workspace hf_align_pad_blend_workspace_bytes(Hp, Wp) of the padded size.
+ * 13 launches: pad, two blur axes, median init and 4 x (histogram, select), blend. */
+size_t hf_align_pad_blend_workspace_bytes(int Hp, int Wp);
+int hf_align_pad_blend_u8(const uint8_t* src, int H, int W, int src_pitch, const int* pad, const double* weights,
+                          int radius, uint8_t* dst, void* workspace, void* stream);
+/* Its stages on their own: gaussian_filter(x, [s, s, 0]) of x, y [Hp][Wp][3] float32 (workspace Hp Wp 3 floats), and
+ * np.median(x, axis=(0, 1)) of x [pixels][3] float32 into med[3] (workspace hf_align_median_workspace_bytes()). */
+int hf_align_gaussian_f32(const float* x, float* y, int Hp, int Wp, const double* weights, int radius,
+                          float* workspace, void* stream);
+size_t hf_align_median_workspace_bytes(void);
+int hf_align_median_f32(const float* x, long long pixels, float* med, void* workspace, void* stream);
+/* Image.transform((out_w, out_h), QUAD, data, BILINEAR) of src [H][W]: coeffs (host) = the 8 bilinear coefficients
+ * Pillow derives from the 8 corner values (x0, (ne_x - x0) / w, ..., see face_align.quad_coefficients). */
+int hf_align_quad_u8(const uint8_t* src, int H, int W, int src_pitch, const double* coeffs, uint8_t* dst, int out_w,
+                     int out_h, void* stream);
+
 /* Number of kernels the last hf_generator_forward / hf_conv_forward of this thread launched. */
 int hf_last_launch_count(void);
 /* Number of kernels every hf_* call of this thread has launched since the library was loaded. */
