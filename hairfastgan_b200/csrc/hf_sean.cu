@@ -285,10 +285,10 @@ using namespace hf;
 extern "C" {
 
 int hf_sean_labels(const long long* labels, int8_t* maps, int* bad, int size, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
   HF_REQUIRE(labels && maps && bad, "hf_sean_labels: null pointer");
   HF_REQUIRE(size >= 32 && size % 32 == 0 && size <= 4096, "hf_sean_labels: size %d must be a multiple of 32", size);
+  int rc = ensure_device_current();
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   HF_CUDA_OK(cudaMemsetAsync(bad, 0, sizeof(int), st));
   sean_labels_kernel<<<grid_for((int64_t)size * size), 256, 0, st>>>(labels, maps, bad, size, 6);
@@ -300,12 +300,12 @@ int hf_sean_labels(const long long* labels, int8_t* maps, int* bad, int size, vo
 int hf_sean_onehot_conv(const int8_t* labels, const float* table, const float* bias, int act, void* y16, int res,
                         int channels, int dtype, void* stream) {
   return with_dtype(dtype, "hf_sean_onehot_conv", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     HF_REQUIRE(labels && table && y16, "hf_sean_onehot_conv: null pointer");
     HF_REQUIRE(res > 0 && channels > 0 && channels % 8 == 0, "hf_sean_onehot_conv: bad shape %d^2 x %d", res, channels);
     HF_REQUIRE(act == 0 || act == 3, "hf_sean_onehot_conv: act %d (0 none, 3 ReLU)", act);
     HF_REQUIRE(((uintptr_t)table & 15) == 0 && ((uintptr_t)y16 & 15) == 0, "hf_sean_onehot_conv: unaligned pointer");
+    int rc = ensure_device_current();
+    if (rc) return rc;
     const int64_t total = (int64_t)res * res * (channels / 8);
     sean_onehot_kernel<dt><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(labels, table, bias, act, (uint16_t*)y16,
                                                                               res, channels / 8);
@@ -317,10 +317,10 @@ int hf_sean_onehot_conv(const int8_t* labels, const float* table, const float* b
 
 int hf_sean_style_tables(const float* image_code, const float* mean_code, const hf_sean_ace_tables* aces, int n_ace,
                          float* mu_workspace, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
   HF_REQUIRE(image_code && mean_code && aces && mu_workspace, "hf_sean_style_tables: null pointer");
   HF_REQUIRE(n_ace >= 1 && n_ace <= kMaxAce, "hf_sean_style_tables: %d ACE layers (1..%d)", n_ace, kMaxAce);
+  HF_REQUIRE(aligned16(image_code, mean_code, mu_workspace),
+             "hf_sean_style_tables: image_code, mean_code and mu_workspace must be 16-byte aligned");
   SeanAceJobs jobs;
   memset(&jobs, 0, sizeof(jobs));
   int blocks = 0;
@@ -328,9 +328,12 @@ int hf_sean_style_tables(const float* image_code, const float* mean_code, const 
     const hf_sean_ace_tables& s = aces[a];
     HF_REQUIRE(s.fc_w && s.fc_b && s.tw && s.table, "hf_sean_style_tables: null pointer in ACE %d", a);
     HF_REQUIRE(s.n2 > 0 && s.n2 % 8 == 0, "hf_sean_style_tables: ACE %d width %d", a, s.n2);
+    HF_REQUIRE(aligned16(s.fc_w, s.tw), "hf_sean_style_tables: fc_w and tw of ACE %d must be 16-byte aligned", a);
     jobs.job[a] = SeanAceJob{s.fc_w, s.fc_b, s.tw, s.table, s.n2, blocks};
     blocks += (9 * s.n2 + 7) / 8;
   }
+  int rc = ensure_device_current();
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   sean_fc_mu_kernel<<<dim3(kStyle / 8, kClasses, n_ace), 256, 0, st>>>(image_code, mean_code, jobs, mu_workspace);
   HF_LAUNCH_OK("sean_fc_mu");
@@ -344,14 +347,14 @@ int hf_sean_ace_apply(const void* x16, const float* noise, const float* noise_va
                       const float* bn_shift, const float* gamma_beta, const float* table, const int8_t* labels,
                       int lrelu, void* y16, int res, int channels, int dtype, void* stream) {
   return with_dtype(dtype, "hf_sean_ace_apply", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     HF_REQUIRE(x16 && noise && noise_var && bn_scale && bn_shift && gamma_beta && y16 && (!table || labels),
                "hf_sean_ace_apply: null pointer");
     HF_REQUIRE(res > 0 && res * res % 32 == 0 && channels % 64 == 0 && channels > 0,
                "hf_sean_ace_apply: bad shape %d^2 x %d (pixels %% 32, channels %% 64)", res, channels);
     HF_REQUIRE(((uintptr_t)x16 & 15) == 0 && ((uintptr_t)y16 & 15) == 0 && ((uintptr_t)table & 15) == 0,
                "hf_sean_ace_apply: unaligned pointer");
+    int rc = ensure_device_current();
+    if (rc) return rc;
     const dim3 grid(res * res / 32, channels / 64);
     sean_ace_kernel<dt><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x16, noise, noise_var, bn_scale,
                                                                 bn_shift, gamma_beta, table, labels, lrelu,
@@ -364,11 +367,11 @@ int hf_sean_ace_apply(const void* x16, const float* noise, const float* noise_va
 
 int hf_sean_class_means(const float* y, const int8_t* labels, long long label_stride, float* codes, int batch,
                         int channels, int hw, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
   HF_REQUIRE(y && labels && codes, "hf_sean_class_means: null pointer");
   HF_REQUIRE(batch > 0 && batch <= 65535 && channels > 0 && hw > 0 && label_stride >= hw,
              "hf_sean_class_means: bad shape B=%d C=%d HW=%d label stride %lld", batch, channels, hw, label_stride);
+  int rc = ensure_device_current();
+  if (rc) return rc;
   sean_class_means_kernel<<<dim3(channels, batch), kMeanThreads, 0, (cudaStream_t)stream>>>(y, labels, label_stride,
                                                                                            codes, channels, hw);
   HF_LAUNCH_OK("sean_class_means");
@@ -379,11 +382,12 @@ int hf_sean_class_means(const float* y, const int8_t* labels, long long label_st
 int hf_sean_conv_img(const void* x16, const float* weight, const float* bias, float* y, int res, int channels,
                      int dtype, void* stream) {
   return with_dtype(dtype, "hf_sean_conv_img", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     HF_REQUIRE(x16 && weight && bias && y, "hf_sean_conv_img: null pointer");
     HF_REQUIRE(res > 0 && channels > 0 && channels % 8 == 0 && channels <= kImgMaxC,
                "hf_sean_conv_img: bad shape %d^2 x %d (channels %% 8, <= %d)", res, channels, kImgMaxC);
+    HF_REQUIRE(aligned16(x16), "hf_sean_conv_img: x16 must be 16-byte aligned");
+    int rc = ensure_device_current();
+    if (rc) return rc;
     const int grid = (res * res + 255) / 256;
     sean_conv_img_kernel<dt><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x16, weight, bias, y, res,
                                                                      channels);

@@ -221,10 +221,10 @@ using namespace hf;
 extern "C" {
 
 int hf_shape_labels(long long* mask, int8_t* labels, int* bad, int n, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
   HF_REQUIRE(mask && labels && bad, "hf_shape_labels: null pointer");
   HF_REQUIRE(n > 0, "hf_shape_labels: %d pixels", n);
+  int rc = ensure_device_current();
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   HF_CUDA_OK(cudaMemsetAsync(bad, 0, sizeof(int), st));
   shape_labels_kernel<<<grid_for(n), 256, 0, st>>>(mask, labels, bad, n);
@@ -236,12 +236,12 @@ int hf_shape_labels(long long* mask, int8_t* labels, int* bad, int n, void* stre
 int hf_shape_onehot_s2(const int8_t* labels, const float* table, const float* cmap, void* y16, int res, int channels,
                        int dtype, void* stream) {
   return with_dtype(dtype, "hf_shape_onehot_s2", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     HF_REQUIRE(labels && table && cmap && y16, "hf_shape_onehot_s2: null pointer");
     HF_REQUIRE(res > 0 && channels > 0 && channels % 8 == 0, "hf_shape_onehot_s2: bad shape %d^2 x %d", res, channels);
     HF_REQUIRE(((uintptr_t)table & 15) == 0 && ((uintptr_t)cmap & 15) == 0 && ((uintptr_t)y16 & 15) == 0,
                "hf_shape_onehot_s2: unaligned pointer");
+    int rc = ensure_device_current();
+    if (rc) return rc;
     const int64_t total = (int64_t)res * res * (channels / 8);
     shape_onehot_s2_kernel<dt><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(labels, table, cmap, (uint16_t*)y16,
                                                                                   res, channels / 8);
@@ -271,13 +271,13 @@ size_t hf_shape_gemm_workspace_bytes(int mode, int cin, int cout, int hin, int w
 int hf_shape_gemm(int mode, const void* w16, const void* x16, const float* bias, float* y32, void* y16, float* workspace,
                   int cin, int cout, int hin, int win, int dtype, void* stream) {
   return with_dtype(dtype, "hf_shape_gemm", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     HF_REQUIRE(w16 && x16 && workspace && (y32 || y16), "hf_shape_gemm: null pointer");
     HF_REQUIRE(((uintptr_t)w16 & 15) == 0 && ((uintptr_t)x16 & 15) == 0, "hf_shape_gemm: unaligned operand");
     HF_REQUIRE(cout > 0, "hf_shape_gemm: cout %d", cout);
     GemmShape g;
-    if ((rc = gemm_shape(mode, cin, hin, win, &g))) return rc;
+    int rc = gemm_shape(mode, cin, hin, win, &g);
+    if (rc) return rc;
+    if ((rc = ensure_device_current())) return rc;
     int pl[5];
     gemm_plan(g, cout, num_sms(), pl);
     cudaStream_t st = (cudaStream_t)stream;
@@ -303,13 +303,13 @@ size_t hf_shape_layer_norm_workspace_bytes(long long n) {
 int hf_shape_layer_norm_lrelu(const void* x16, const float* gamma, const float* beta, void* y16, float* workspace,
                               int pixels, int channels, float slope, int dtype, void* stream) {
   return with_dtype(dtype, "hf_shape_layer_norm_lrelu", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     HF_REQUIRE(x16 && gamma && beta && y16 && workspace, "hf_shape_layer_norm_lrelu: null pointer");
     HF_REQUIRE(pixels > 0 && channels > 0 && channels % 8 == 0 && (int64_t)pixels * channels > 1,
                "hf_shape_layer_norm_lrelu: bad shape %d x %d (channels %% 8)", pixels, channels);
     HF_REQUIRE(((uintptr_t)x16 & 15) == 0 && ((uintptr_t)y16 & 15) == 0,
                "hf_shape_layer_norm_lrelu: unaligned pointer");
+    int rc = ensure_device_current();
+    if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t n8 = (int64_t)pixels * channels / 8;
     const int G = ln_blocks(n8);
@@ -330,12 +330,12 @@ int hf_shape_layer_norm_lrelu(const void* x16, const float* gamma, const float* 
 int hf_shape_logits_argmax(const void* hair16, const void* face16, const float* table, const float* bias,
                            long long* labels, int res, int dtype, void* stream) {
   return with_dtype(dtype, "hf_shape_logits_argmax", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     HF_REQUIRE(hair16 && face16 && table && bias && labels, "hf_shape_logits_argmax: null pointer");
     HF_REQUIRE(res > 0 && res <= 4096, "hf_shape_logits_argmax: res %d", res);
     HF_REQUIRE(((uintptr_t)hair16 & 15) == 0 && ((uintptr_t)face16 & 15) == 0,
                "hf_shape_logits_argmax: unaligned input");
+    int rc = ensure_device_current();
+    if (rc) return rc;
     const int grid = (res * res + 255) / 256;
     shape_logits_argmax_kernel<dt><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)hair16,
                                                                            (const uint16_t*)face16, table, bias,

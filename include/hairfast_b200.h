@@ -387,7 +387,8 @@ typedef struct {
 /* Per-call style tables of n_ace (<= 16) ACE layers in two launches:
  * code_j = image_code[j] ([19][512]) unless that row is all zero, then mean_code[j] (pix2pix_model.py:312-315);
  * mu_j = relu(fc_w[j] . code_j + fc_b[j]) (normalization.py:133-135); table[j][tap][n] = tw[tap*n2 + n] . mu_j.
- * aces: HOST array; mu_workspace: n_ace * 19 * 512 floats. */
+ * aces: HOST array; mu_workspace: n_ace * 19 * 512 floats.  image_code, mean_code, mu_workspace and every ACE's fc_w
+ * and tw are read with 16-byte loads: each must be 16-byte aligned. */
 int hf_sean_style_tables(const float* image_code, const float* mean_code, const hf_sean_ace_tables* aces, int n_ace,
                          float* mu_workspace, void* stream);
 
@@ -401,7 +402,7 @@ int hf_sean_ace_apply(const void* x16, const float* noise, const float* noise_va
                       int lrelu, void* y16, int res, int channels, int dtype, void* stream);
 
 /* tanh(conv_img(leaky_relu(x, 0.2))) (generator.py:107-108): x16 [res,res,channels] 16-bit NHWC, weight [3][channels]
- * [3][3], bias [3] -> y [3,res,res] fp32 NCHW.  channels % 8 == 0, <= 256. */
+ * [3][3], bias [3] -> y [3,res,res] fp32 NCHW.  channels % 8 == 0, <= 256; x16 16-byte aligned. */
 int hf_sean_conv_img(const void* x16, const float* weight, const float* bias, float* y, int res, int channels,
                      int dtype, void* stream);
 

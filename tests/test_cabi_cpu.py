@@ -97,6 +97,53 @@ def test_unaligned_16bit_tensors_rejected_without_device(lib, dt):
 
 
 @no_device_only
+@pytest.mark.parametrize("dt", ["HF_BF16", "HF_F16"])
+def test_sean_and_shape_unaligned_operands_rejected_without_device(lib, dt):
+    """The SEAN and shape adaptor entry points check every operand their kernels read or write 16 bytes at a time
+    (uint4 for 16-bit tensors, float4 for fp32 rows) before any device call: an fp32 pointer that is only 4-byte
+    aligned (0x...4) or a 16-bit one that is only 8-byte aligned (0x...8) is an error, not a launch."""
+    h, d = lib.lib(), getattr(lib, dt)
+    A, B_, C_, D_, E, U4, U8 = 0x10000, 0x20000, 0x30000, 0x40000, 0x60000, 0x50004, 0x50008
+
+    def aces(fc_w, tw):
+        arr = (lib.hf_sean_ace_tables * 2)()
+        arr[0] = lib.hf_sean_ace_tables(A, B_, C_, D_, 64)
+        arr[1] = lib.hf_sean_ace_tables(fc_w, B_, tw, D_, 64)
+        return arr
+
+    tables = b"hf_sean_style_tables: image_code, mean_code and mu_workspace must be 16-byte aligned"
+    ace_rows = b"hf_sean_style_tables: fc_w and tw of ACE 1 must be 16-byte aligned"
+    cases = [
+        (h.hf_sean_conv_img, (U8, A, B_, C_, 4, 8, d, None), b"hf_sean_conv_img: x16 must be 16-byte aligned"),
+        (h.hf_sean_style_tables, (U4, A, aces(A, A), 2, B_, None), tables),
+        (h.hf_sean_style_tables, (A, U4, aces(A, A), 2, B_, None), tables),
+        (h.hf_sean_style_tables, (A, B_, aces(A, A), 2, U4, None), tables),
+        (h.hf_sean_style_tables, (A, B_, aces(U4, A), 2, C_, None), ace_rows),
+        (h.hf_sean_style_tables, (A, B_, aces(A, U4), 2, C_, None), ace_rows),
+        (h.hf_sean_onehot_conv, (A, U4, None, 0, B_, 8, 8, d, None), b"hf_sean_onehot_conv: unaligned pointer"),
+        (h.hf_sean_onehot_conv, (A, B_, None, 0, U8, 8, 8, d, None), b"hf_sean_onehot_conv: unaligned pointer"),
+        (h.hf_sean_ace_apply, (U8, A, A, A, A, A, None, None, 0, B_, 8, 64, d, None), b"hf_sean_ace_apply: unaligned"),
+        (h.hf_sean_ace_apply, (A, A, A, A, A, A, None, None, 0, U8, 8, 64, d, None), b"hf_sean_ace_apply: unaligned"),
+        (h.hf_sean_ace_apply, (A, A, A, A, A, A, U4, B_, 0, C_, 8, 64, d, None), b"hf_sean_ace_apply: unaligned"),
+        (h.hf_shape_onehot_s2, (A, U4, B_, C_, 4, 8, d, None), b"hf_shape_onehot_s2: unaligned pointer"),
+        (h.hf_shape_onehot_s2, (A, B_, U4, C_, 4, 8, d, None), b"hf_shape_onehot_s2: unaligned pointer"),
+        (h.hf_shape_onehot_s2, (A, B_, C_, U8, 4, 8, d, None), b"hf_shape_onehot_s2: unaligned pointer"),
+        (h.hf_shape_layer_norm_lrelu, (U8, A, A, B_, C_, 4, 8, 0.2, d, None), b"hf_shape_layer_norm_lrelu: unaligned"),
+        (h.hf_shape_layer_norm_lrelu, (A, B_, B_, U8, C_, 4, 8, 0.2, d, None), b"hf_shape_layer_norm_lrelu: unaligned"),
+        (h.hf_shape_logits_argmax, (U8, A, B_, C_, D_, 4, d, None), b"hf_shape_logits_argmax: unaligned input"),
+        (h.hf_shape_logits_argmax, (A, U8, B_, C_, D_, 4, d, None), b"hf_shape_logits_argmax: unaligned input"),
+        (h.hf_shape_gemm, (0, U8, A, None, B_, None, C_, 8, 8, 4, 4, d, None), b"hf_shape_gemm: unaligned operand"),
+        (h.hf_shape_gemm, (0, A, U8, None, B_, None, C_, 8, 8, 4, 4, d, None), b"hf_shape_gemm: unaligned operand"),
+    ]
+    for fn, args, msg in cases:
+        assert fn(*args) == -1, (fn.__name__, args)                   # HF_ERR_INVALID
+        assert h.hf_last_error().startswith(msg), (fn.__name__, args, h.hf_last_error())
+    for n_ace in (0, 17):                                                 # 1..16 ACE layers per call
+        assert h.hf_sean_style_tables(A, B_, aces(A, A), n_ace, C_, None) == -1
+        assert b"ACE layers (1..16)" in h.hf_last_error(), h.hf_last_error()
+
+
+@no_device_only
 def test_unaligned_style_rows_rejected_without_device(lib):
     """The style affine reads latent rows and modulation weights with float4 loads: hf_torgb_forward,
     hf_conv_forward and hf_generator_forward reject a pointer that is only 4-byte aligned (0x...4), before any
