@@ -447,10 +447,9 @@ int hf_mod_gemm_plan(const hf_mod_desc* d, int batch, int layer, int sms, int* o
 int hf_mod_embed16(const hf_mod_desc* d, int batch, const hf_mod_rows* src, void* e16, void* stream) {
   HF_REQUIRE(d, "hf_mod_embed16: null descriptor");
   return with_dtype(d->dtype, "hf_mod_embed16", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     Desc m;
-    if ((rc = check_desc(d, batch, "hf_mod_embed16", &m))) return rc;
+    int rc = check_desc(d, batch, "hf_mod_embed16", &m);
+    if (rc) return rc;
     HF_REQUIRE(src && e16 && aligned16(e16), "hf_mod_embed16: null or unaligned pointer");
     Sources s{};
     const int n = m.inp / kDim * m.stacks;
@@ -458,6 +457,7 @@ int hf_mod_embed16(const hf_mod_desc* d, int batch, const hf_mod_rows* src, void
       HF_REQUIRE(src[i].ptr, "hf_mod_embed16: source %d is null", i);
       s.r[i] = src[i];
     }
+    if ((rc = ensure_device_current())) return rc;
     const int64_t total = (int64_t)m.stacks * m.rows * m.inp / 8;
     mod_embed16_kernel<dt><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(s, (uint16_t*)e16, m.L, m.rows, m.inp,
                                                                              m.stacks);
@@ -471,13 +471,13 @@ int hf_mod_gemm(const hf_mod_desc* d, int batch, int layer, const void* w16, con
                 float* y32, float* workspace, void* stream) {
   HF_REQUIRE(d, "hf_mod_gemm: null descriptor");
   return with_dtype(d->dtype, "hf_mod_gemm", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     Desc m;
     StyleGemm sg;
+    int rc;
     if ((rc = check_desc(d, batch, "hf_mod_gemm", &m)) || (rc = style_gemm(m, layer, "hf_mod_gemm", &sg))) return rc;
     HF_REQUIRE(w16 && x16 && y32 && workspace, "hf_mod_gemm: null pointer");
     HF_REQUIRE(aligned16(w16) && aligned16(x16), "hf_mod_gemm: unaligned operand");
+    if ((rc = ensure_device_current())) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     int pl[5];
     if ((rc = run_style_gemm<dt>(sg, w16, x16, workspace, st, pl))) return rc;
@@ -493,13 +493,14 @@ int hf_mod_hidden(const hf_mod_desc* d, int batch, const void* w16, const void* 
                   const float* ln_w, const float* ln_b, void* h16, float* workspace, void* stream) {
   HF_REQUIRE(d, "hf_mod_hidden: null descriptor");
   return with_dtype(d->dtype, "hf_mod_hidden", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     Desc m;
     StyleGemm sg;
+    int rc;
     if ((rc = check_desc(d, batch, "hf_mod_hidden", &m)) || (rc = style_gemm(m, 1, "hf_mod_hidden", &sg))) return rc;
     HF_REQUIRE(w16 && e16 && bias && ln_w && ln_b && h16 && workspace, "hf_mod_hidden: null pointer");
     HF_REQUIRE(aligned16(w16) && aligned16(e16), "hf_mod_hidden: unaligned operand");
+    HF_REQUIRE(((uintptr_t)h16 & 1) == 0, "hf_mod_hidden: h16 must be 2-byte aligned");
+    if ((rc = ensure_device_current())) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     int pl[5];
     if ((rc = run_style_gemm<dt>(sg, w16, e16, workspace, st, pl))) return rc;
@@ -515,20 +516,18 @@ int hf_mod_chain(const hf_mod_desc* d, int batch, const void* fc_w16, const floa
                  const hf_mod_rows* x0, const hf_mod_rows* base, float* out, float* workspace, void* stream) {
   HF_REQUIRE(d, "hf_mod_chain: null descriptor");
   return with_dtype(d->dtype, "hf_mod_chain", [&](auto dt) -> int {
-    int rc = ensure_device_current();
-    if (rc) return rc;
     Desc m;
-    if ((rc = check_desc(d, batch, "hf_mod_chain", &m))) return rc;
+    int rc = check_desc(d, batch, "hf_mod_chain", &m);
+    if (rc) return rc;
     HF_REQUIRE(fc_w16 && fc_b && gb && x0 && base && base->ptr && out && workspace, "hf_mod_chain: null pointer");
     HF_REQUIRE(aligned16(fc_w16), "hf_mod_chain: unaligned weights");
+    for (int s = 0; s < m.stacks; ++s) HF_REQUIRE(x0[s].ptr, "hf_mod_chain: x0[%d] is null", s);
+    if ((rc = ensure_device_current())) return rc;
     ChainArgs a{};
     a.w = (const uint16_t*)fc_w16;
     a.bias = fc_b;
     a.gb = gb;
-    for (int s = 0; s < m.stacks; ++s) {
-      HF_REQUIRE(x0[s].ptr, "hf_mod_chain: x0[%d] is null", s);
-      a.x0[s] = x0[s];
-    }
+    for (int s = 0; s < m.stacks; ++s) a.x0[s] = x0[s];
     a.base = *base;
     a.out = out;
     a.dt = workspace;

@@ -475,26 +475,28 @@ size_t hf_mod_workspace_bytes(const hf_mod_desc* d, int batch);
 /* The split-K plan of style layer 1 or 2 on a device with `sms` SMs (needs no device): out[5] = {row tile, K splits,
  * 64-wide K tiles, output tiles, row tiles}. */
 int hf_mod_gemm_plan(const hf_mod_desc* d, int batch, int layer, int sms, int* out);
-/* The 16-bit embedding e16 [stacks][rows][inp]: stack s's columns 512 j .. 512 j + 511 are src[s * inp / 512 + j]. */
+/* The 16-bit embedding e16 [stacks][rows][inp]: stack s's columns 512 j .. 512 j + 511 are src[s * inp / 512 + j].
+ * e16 must be 16-byte aligned. */
 int hf_mod_embed16(const hf_mod_desc* d, int batch, const hf_mod_rows* src, void* e16, void* stream);
 /* Grouped split-K GEMM of style layer 1 or 2, y32 = x16 w16^T + bias, partials added in split order:
  *   layer 1: stacks groups, w16 [stacks][10 middle][inp], x16 = e16 [stacks][rows][inp], bias [stacks][10 middle],
  *            y32 [stacks][rows][10 middle];
  *   layer 2: 10 stacks groups, w16 [10 stacks][512][middle], x16 = h16 [rows][10 stacks middle] (group g reads
  *            columns g middle ..), bias [10 stacks][512], y32 = gamma / beta [10 stacks][rows][512].
- * bias may be NULL. */
+ * bias may be NULL.  w16 and x16 must be 16-byte aligned. */
 int hf_mod_gemm(const hf_mod_desc* d, int batch, int layer, const void* w16, const void* x16, const float* bias,
                 float* y32, float* workspace, void* stream);
 /* Style layer 1 with the rest of Linear -> LayerNorm([middle]) -> LeakyReLU(0.01) fused into its reduction:
  * h16[p][(s 10 + j) middle + n] for branch j of stack s; bias [stacks][10 middle], ln_w / ln_b [stacks][10][middle]
- * (biased variance, eps 1e-5). */
+ * (biased variance, eps 1e-5).  w16 and e16 must be 16-byte aligned, h16 2-byte aligned. */
 int hf_mod_hidden(const hf_mod_desc* d, int batch, const void* w16, const void* e16, const float* bias,
                   const float* ln_w, const float* ln_b, void* h16, float* workspace, void* stream);
 /* The fc chain on thread-block clusters of 8 CTAs per (stack, sample): PixelNorm over the layers of x0[s], then per
  * module fc (fc_w16 [stacks][5][512][512], fc_b [stacks][5][512]), LayerNorm over the whole [layers, 512] sample,
  * x (1 + gamma) + beta (gb from hf_mod_gemm layer 2) and LeakyReLU(0.01) except after the last module.
  * out [batch][layers][512] = base + 0.1 dt for one stack, base + 0.1 (dt_0 + dt_1) for two.  One kernel launch; with
- * two stacks it is preceded by a cudaMemsetAsync of the completion counters in the workspace. */
+ * two stacks it is preceded by a cudaMemsetAsync of the completion counters in the workspace.  fc_w16 must be 16-byte
+ * aligned. */
 int hf_mod_chain(const hf_mod_desc* d, int batch, const void* fc_w16, const float* fc_b, const float* gb,
                  const hf_mod_rows* x0, const hf_mod_rows* base, float* out, float* workspace, void* stream);
 

@@ -406,3 +406,43 @@ def test_conv_plans_for_every_generator_layer(lib):
             assert work == n_n * -(-batch * r * r // 128) if r >= 16 else work >= n_n
             if up:
                 assert n_tile == 128
+
+
+@no_device_only
+@pytest.mark.parametrize("dt", ["HF_BF16", "HF_F16"])
+def test_modulation_arguments_checked_without_device(lib, dt):
+    """hf_mod_embed16, hf_mod_gemm, hf_mod_hidden and hf_mod_chain check the descriptor, NULL pointers and the
+    alignment of every pointer their kernels reach wider than its type (16-byte cp.async / uint4 operands, the 2-byte
+    hidden rows) before they select a device or launch."""
+    h, d16 = lib.lib(), getattr(lib, dt)
+    A, B_, C_, D_, E, U8, U1 = 0x10000, 0x20000, 0x30000, 0x40000, 0x60000, 0x50008, 0x50001
+    d = lib.hf_mod_desc(6, 512, 512, 1, d16)
+    bad = lib.hf_mod_desc(25, 512, 512, 1, d16)
+    src = (lib.hf_mod_rows * 1)(lib.hf_mod_rows(A, 6 * 512, 512))
+    nul = (lib.hf_mod_rows * 1)(lib.hf_mod_rows(None, 0, 0))
+    x0 = (lib.hf_mod_rows * 2)(lib.hf_mod_rows(A, 6 * 512, 512), lib.hf_mod_rows(A, 6 * 512, 512))
+    x0n = (lib.hf_mod_rows * 2)(lib.hf_mod_rows(None, 0, 0), lib.hf_mod_rows(None, 0, 0))
+    base = lib.hf_mod_rows(B_, 0, 512)
+    r = C.byref
+    cases = [
+        (h.hf_mod_embed16, (r(bad), 1, src, A, None), b"hf_mod_embed16: layers 25"),
+        (h.hf_mod_embed16, (r(d), 0, src, A, None), b"hf_mod_embed16: batch 0"),
+        (h.hf_mod_embed16, (r(d), 1, src, U8, None), b"hf_mod_embed16: null or unaligned pointer"),
+        (h.hf_mod_embed16, (r(d), 1, nul, A, None), b"hf_mod_embed16: source 0 is null"),
+        (h.hf_mod_gemm, (r(d), 1, 3, A, B_, None, C_, D_, None), b"hf_mod_gemm: layer 3"),
+        (h.hf_mod_gemm, (r(d), 1, 2, A, B_, None, None, D_, None), b"hf_mod_gemm: null pointer"),
+        (h.hf_mod_gemm, (r(d), 1, 1, U8, B_, None, C_, D_, None), b"hf_mod_gemm: unaligned operand"),
+        (h.hf_mod_gemm, (r(d), 1, 2, A, U8, None, C_, D_, None), b"hf_mod_gemm: unaligned operand"),
+        (h.hf_mod_hidden, (r(bad), 1, A, B_, C_, C_, C_, D_, E, None), b"hf_mod_hidden: layers 25"),
+        (h.hf_mod_hidden, (r(d), 1, A, B_, None, C_, C_, D_, E, None), b"hf_mod_hidden: null pointer"),
+        (h.hf_mod_hidden, (r(d), 1, U8, B_, C_, C_, C_, D_, E, None), b"hf_mod_hidden: unaligned operand"),
+        (h.hf_mod_hidden, (r(d), 1, A, U8, C_, C_, C_, D_, E, None), b"hf_mod_hidden: unaligned operand"),
+        (h.hf_mod_hidden, (r(d), 1, A, B_, C_, C_, C_, U1, E, None), b"hf_mod_hidden: h16 must be 2-byte aligned"),
+        (h.hf_mod_chain, (r(bad), 1, A, B_, C_, x0, r(base), D_, E, None), b"hf_mod_chain: layers 25"),
+        (h.hf_mod_chain, (r(d), 1, A, B_, C_, x0, r(base), None, E, None), b"hf_mod_chain: null pointer"),
+        (h.hf_mod_chain, (r(d), 1, U8, B_, C_, x0, r(base), D_, E, None), b"hf_mod_chain: unaligned weights"),
+        (h.hf_mod_chain, (r(d), 1, A, B_, C_, x0n, r(base), D_, E, None), b"hf_mod_chain: x0[0] is null"),
+    ]
+    for fn, args, msg in cases:
+        assert fn(*args) == -1, (fn.__name__, args)                   # HF_ERR_INVALID
+        assert h.hf_last_error().startswith(msg), (fn.__name__, args, h.hf_last_error())
