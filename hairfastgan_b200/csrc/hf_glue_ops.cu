@@ -90,7 +90,8 @@ __global__ void __launch_bounds__(256) dilate_erode_step_kernel(const float* __r
 // `F.interpolate(mode='bicubic')` = PyTorch's upsample_bicubic2d, align_corners=False, A = -0.75: source coordinate
 // (i + 0.5) * in / out - 0.5, four taps around its floor with clamped indices.  One launch: every CTA first evaluates
 // the n_stage interpolated weights of its 256 pixels (shared memory), then streams its channel slice with 16-byte
-// accesses.  fp32 throughout; the only difference from the torch expression is fma contraction (<= 1e-6).
+// accesses (4-byte ones when P % 4 != 0, past the last full quad, or when a tensor is not 16-byte aligned).  fp32
+// throughout; the only difference from the torch expression is fma contraction (<= 1e-6).
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) align_masks_kernel(const float* __restrict__ hm1, const float* __restrict__ hm2,
                                                           const float* __restrict__ hmx, float* __restrict__ out,
@@ -120,6 +121,7 @@ struct BlendArgs {
   float scale_a[kBlendMaxStage], scale_b[kBlendMaxStage];
   float* out;                          // [C, P]
   int n_stage, C, Ho, Wo, Hm, Wm, ch_per_block;
+  int aligned;                         // first, every src[s] and out 16-byte aligned: the float4 path may run
 };
 
 __global__ void __launch_bounds__(256) fspace_blend_kernel(const BlendArgs a) {
@@ -154,7 +156,7 @@ __global__ void __launch_bounds__(256) fspace_blend_kernel(const BlendArgs a) {
   const int c0 = blockIdx.y * a.ch_per_block, c1 = min(c0 + a.ch_per_block, a.C);
   // 64 threads x float4 cover the 256 pixels of this CTA; 4 channel rows in flight per pass
   const int lane4 = (threadIdx.x & 63) * 4, crow = threadIdx.x >> 6;
-  const bool vec = (P % 4 == 0) && (p0 + lane4 + 3 < P);
+  const bool vec = a.aligned && (P % 4 == 0) && (p0 + lane4 + 3 < P);
   for (int c = c0 + crow; c < c1; c += 4) {
     const size_t off = (size_t)c * P + p0 + lane4;
     if (vec) {
@@ -188,14 +190,14 @@ extern "C" {
 
 int hf_bicubic_downsample_f32(const float* x, const float* k, float* y, int planes, int H, int W, int factor,
                               int clip_round, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
   HF_REQUIRE(x && k && y, "bicubic_down: null pointer");
   HF_REQUIRE(factor >= 1 && factor <= kBicMaxFactor, "bicubic_down: factor %d unsupported (1..%d)", factor, kBicMaxFactor);
   HF_REQUIRE(planes > 0 && planes <= 65535 && H > 0 && W > 0, "bicubic_down: bad shape");
   const int taps = 4 * factor, pad = taps - factor;
   HF_REQUIRE(pad / 2 < H && pad - pad / 2 < H && pad / 2 < W && pad - pad / 2 < W, "bicubic_down: image smaller than the reflect padding");
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
   const int Ho = (H + pad - taps) / factor + 1, Wo = (W + pad - taps) / factor + 1;
   const size_t smem = (size_t)(4 * kBicMaxFactor + kBicTileH * (kBicTileW * factor + pad)) * sizeof(float);
   dim3 grid((Wo + kBicTileW - 1) / kBicTileW, (Ho + kBicTileH - 1) / kBicTileH, planes);
@@ -207,21 +209,21 @@ int hf_bicubic_downsample_f32(const float* x, const float* k, float* y, int plan
 
 int hf_dilate_erode_f32(const float* mask, float* dilate, float* erode, void* workspace, int planes, int H, int W,
                         int iterations, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
   float* ws = (float*)workspace;
   HF_REQUIRE(mask && dilate && erode, "dilate_erode: null pointer");
   HF_REQUIRE(planes > 0 && H > 0 && W > 0 && iterations >= 0, "dilate_erode: bad arguments");
   const int64_t total = (int64_t)planes * H * W;
   HF_REQUIRE(total < (int64_t)2000000000, "dilate_erode: tensor too large for one launch");
+  HF_REQUIRE(iterations <= 1 || ws, "dilate_erode: workspace (2 planes sets) needed for more than one iteration");
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
   const size_t bytes = (size_t)total * sizeof(float);
   if (iterations == 0) {
     HF_CUDA_OK(cudaMemcpyAsync(dilate, mask, bytes, cudaMemcpyDeviceToDevice, st));
     HF_CUDA_OK(cudaMemcpyAsync(erode, mask, bytes, cudaMemcpyDeviceToDevice, st));
     return HF_OK;
   }
-  HF_REQUIRE(iterations == 1 || ws, "dilate_erode: workspace (2 planes sets) needed for more than one iteration");
   const int grid = grid_for(total);
   // buffers: round r reads (d_in, e_in) and writes (d_out, e_out); the last round writes the outputs
   const float *d_in = mask, *e_in = mask;
@@ -240,10 +242,10 @@ int hf_dilate_erode_f32(const float* mask, float* dilate, float* erode, void* wo
 }
 
 int hf_align_masks_f32(const float* hm1, const float* hm2, const float* hmx, float* out, int n, void* stream) {
+  HF_REQUIRE(hm1 && hm2 && hmx && out && n > 0, "align_masks: bad arguments");
   int rc = ensure_device_current();
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  HF_REQUIRE(hm1 && hm2 && hmx && out && n > 0, "align_masks: bad arguments");
   align_masks_kernel<<<(n + 255) / 256, 256, 0, st>>>(hm1, hm2, hmx, out, n);
   HF_LAUNCH_OK("align_masks");
   count_launch();
@@ -253,18 +255,22 @@ int hf_align_masks_f32(const float* hm1, const float* hm2, const float* hmx, flo
 int hf_fspace_blend_f32(const float* first, const float* const* src, const float* const* mask, const float* scale_a,
                         const float* scale_b, float* out, int n_stage, int C, int Ho, int Wo, int Hm, int Wm,
                         void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  HF_REQUIRE(first && src && mask && out, "fspace_blend: null pointer");
+  HF_REQUIRE(first && src && mask && scale_a && scale_b && out, "fspace_blend: null pointer");
   HF_REQUIRE(n_stage >= 1 && n_stage <= kBlendMaxStage, "fspace_blend: 1..%d stages", kBlendMaxStage);
   HF_REQUIRE(C > 0 && Ho > 0 && Wo > 0 && Hm > 0 && Wm > 0, "fspace_blend: bad shape");
   BlendArgs a;
   a.first = first; a.out = out; a.n_stage = n_stage; a.C = C; a.Ho = Ho; a.Wo = Wo; a.Hm = Hm; a.Wm = Wm;
+  uintptr_t bits = (uintptr_t)first | (uintptr_t)out;
   for (int s = 0; s < n_stage; ++s) {
     HF_REQUIRE(src[s] && mask[s], "fspace_blend: null stage pointer");
     a.src[s] = src[s]; a.mask[s] = mask[s]; a.scale_a[s] = scale_a[s]; a.scale_b[s] = scale_b[s];
+    bits |= (uintptr_t)src[s];
   }
+  // contiguous views may start at any 4-byte offset (fspace.py only calls .contiguous()): scalar path then
+  a.aligned = (bits & 15) == 0;
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
   const int P = Ho * Wo;
   a.ch_per_block = 16;
   dim3 grid((P + 255) / 256, (C + a.ch_per_block - 1) / a.ch_per_block);

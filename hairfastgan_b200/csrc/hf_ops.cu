@@ -377,7 +377,8 @@ __global__ void __launch_bounds__(256) bias_act_kernel(const float* __restrict__
     const int64_t n4 = n >> 2;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
       float4 v = __ldg(reinterpret_cast<const float4*>(x) + i);
-      float bb = size_b ? __ldg(b + ((i * 4) / step_b) % size_b) : 0.f;   // step_b % 4 == 0: one channel
+      // step_b % 4 == 0: one channel.  No bias adds -0, the identity of IEEE addition (+0 would turn -0 into +0)
+      float bb = size_b ? __ldg(b + ((i * 4) / step_b) % size_b) : -0.f;
       float r[4] = {v.x + bb, v.y + bb, v.z + bb, v.w + bb};
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
@@ -403,7 +404,7 @@ __global__ void __launch_bounds__(256) bias_act_plane_kernel(const float* __rest
                                                              float* __restrict__ y, int quads_per_plane, int size_b,
                                                              int act, float alpha, float scale) {
   const int plane = blockIdx.y;
-  const float bb = size_b ? __ldg(b + plane % size_b) : 0.f;
+  const float bb = size_b ? __ldg(b + plane % size_b) : -0.f;        // -0: x + bb == x for every x, -0 included
   const float4* xp = reinterpret_cast<const float4*>(x) + (size_t)plane * quads_per_plane;
   float4* yp = reinterpret_cast<float4*>(y) + (size_t)plane * quads_per_plane;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < quads_per_plane; i += gridDim.x * blockDim.x) {
@@ -860,11 +861,8 @@ extern "C" {
 
 int hf_upfirdn2d_f32(const float* x, float* y, const float* k, int planes, int in_h, int in_w, int kh, int kw,
                      int up_x, int up_y, int down_x, int down_y, int px0, int px1, int py0, int py1, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
   reset_launch_count();
   if (planes == 0) return HF_OK;
-  cudaStream_t st = (cudaStream_t)stream;
   HF_REQUIRE(x && y && k, "upfirdn2d: null pointer");
   HF_REQUIRE(planes >= 0 && in_h > 0 && in_w > 0 && kh > 0 && kw > 0, "upfirdn2d: bad shape");
   HF_REQUIRE(up_x > 0 && up_y > 0 && down_x > 0 && down_y > 0, "upfirdn2d: up/down must be positive");
@@ -872,6 +870,9 @@ int hf_upfirdn2d_f32(const float* x, float* y, const float* k, int planes, int i
   const int out_w = (in_w * up_x + px0 + px1 - kw) / down_x + 1;
   HF_REQUIRE(in_h * up_y + py0 + py1 - kh >= 0 && in_w * up_x + px0 + px1 - kw >= 0,
              "upfirdn2d: output would be empty (in %dx%d up %d pad %d,%d k %d)", in_h, in_w, up_y, py0, py1, kh);
+  int rc = ensure_device_current();
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
   const bool k4 = (kh == 4 && kw == 4);
   const bool sym = (up_x == up_y && down_x == down_y);
   const bool pads03 = px0 >= 0 && py0 >= 0 && px1 >= 0 && py1 >= 0 && px0 <= 3 && px1 <= 3 && py0 <= 3 && py1 <= 3;
@@ -910,13 +911,17 @@ int hf_upfirdn2d_f32(const float* x, float* y, const float* k, int planes, int i
 
 int hf_bias_act_f32(const float* x, const float* b, float* y, int64_t n, int size_b, int64_t step_b, int act,
                     float alpha, float scale, void* stream) {
-  int rc = ensure_device_current();
-  if (rc) return rc;
   reset_launch_count();
   if (n == 0) return HF_OK;
+  HF_REQUIRE(x && y, "bias_act: null pointer");
+  HF_REQUIRE(act == 1 || act == 3, "bias_act: act must be 1 (linear) or 3 (leaky relu), got %d", act);
+  HF_REQUIRE(n >= 0 && size_b >= 0 && step_b >= 1, "bias_act: bad sizes");
+  HF_REQUIRE(size_b == 0 || b, "bias_act: bias pointer is null");
+  int rc = ensure_device_current();
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  if (x && y && (size_b == 0 || b) && (act == 1 || act == 3) && step_b % 4 == 0 && step_b >= 1024 && n % step_b == 0 &&
-      n / step_b <= 65535 && step_b / 4 < (int64_t)2000000000 && ((((uintptr_t)x | (uintptr_t)y) & 15) == 0)) {
+  if (step_b % 4 == 0 && step_b >= 1024 && n % step_b == 0 && n / step_b <= 65535 &&
+      step_b / 4 < (int64_t)2000000000 && ((((uintptr_t)x | (uintptr_t)y) & 15) == 0)) {
     const int planes = (int)(n / step_b), quads = (int)(step_b / 4);
     const int gx = std::max(1, std::min(cdiv(quads, 256), std::max(1, num_sms() * 16 / planes)));
     bias_act_plane_kernel<<<dim3(gx, planes), 256, 0, st>>>(x, b, y, quads, size_b, act, alpha, scale);
@@ -924,11 +929,6 @@ int hf_bias_act_f32(const float* x, const float* b, float* y, int64_t n, int siz
     count_launch();
     return HF_OK;
   }
-  HF_REQUIRE(x && y, "bias_act: null pointer");
-  HF_REQUIRE(act == 1 || act == 3, "bias_act: act must be 1 (linear) or 3 (leaky relu), got %d", act);
-  HF_REQUIRE(n >= 0 && size_b >= 0 && step_b >= 1, "bias_act: bad sizes");
-  HF_REQUIRE(size_b == 0 || b, "bias_act: bias pointer is null");
-  if (n == 0) return HF_OK;
   const bool vec = (step_b % 4 == 0) && (n % 4 == 0) && ((((uintptr_t)x | (uintptr_t)y) & 15) == 0);
   const int grid = grid_for(vec ? n / 4 : n);
   if (vec)

@@ -57,7 +57,7 @@ int hf_upfirdn2d_f32(const float* x, float* y, const float* kernel, int planes, 
 /* Replaces fused.fused_bias_act(input, bias, refer, act, grad=0, alpha, scale)
  * (op/fused_bias_act.cpp:11-21, op/fused_bias_act_kernel.cu:19-99), forward only:
  * y[i] = act(x[i] + bias[(i / step_b) % size_b]) * scale; act: 1 = linear, 3 = leaky relu(alpha).
- * bias may be NULL (size_b = 0). */
+ * bias may be NULL (size_b = 0): then nothing is added, so y keeps the sign of a zero x like the reference. */
 int hf_bias_act_f32(const float* x, const float* bias, float* y, int64_t n, int size_b, int64_t step_b,
                     int act, float alpha, float scale, void* stream);
 
@@ -355,7 +355,10 @@ int hf_align_masks_f32(const float* hair_mask1, const float* hair_mask2, const f
  *   F   = src[s] + w_s * (F - src[s])   for s = 0 .. n_stage-1, F starting from `first`
  * first, src[s], out: [channels, height, width] fp32; w_s broadcasts over channels; src / mask are HOST arrays of
  * n_stage device pointers, scale_a / scale_b HOST arrays of n_stage floats (1 <= n_stage <= 4).  Alignment uses
- * (scale_a, scale_b) = (1, -1) (`interpolation_low = 1 - free_mask_down_32`), Embedding (0, opts.mixing). */
+ * (scale_a, scale_b) = (1, -1) (`interpolation_low = 1 - free_mask_down_32`), Embedding (0, opts.mixing).
+ * No pointer needs more than 4-byte alignment: when first, a src[s] or out is not 16-byte aligned the kernel reads and
+ * writes 4 bytes at a time instead of 16.  NULL first, src, mask, scale_a, scale_b, out or a NULL src[s] / mask[s] is
+ * an error. */
 int hf_fspace_blend_f32(const float* first, const float* const* src, const float* const* mask, const float* scale_a,
                         const float* scale_b, float* out, int n_stage, int channels, int height, int width,
                         int mask_height, int mask_width, void* stream);

@@ -446,3 +446,47 @@ def test_modulation_arguments_checked_without_device(lib, dt):
     for fn, args, msg in cases:
         assert fn(*args) == -1, (fn.__name__, args)                   # HF_ERR_INVALID
         assert h.hf_last_error().startswith(msg), (fn.__name__, args, h.hf_last_error())
+
+
+@no_device_only
+def test_stylegan2_op_and_glue_arguments_checked_without_device(lib):
+    """hf_upfirdn2d_f32, hf_bias_act_f32, hf_bicubic_downsample_f32, hf_dilate_erode_f32, hf_align_masks_f32 and
+    hf_fspace_blend_f32 check their arguments before they select a device; empty inputs are no-ops."""
+    h = lib.lib()
+    A, B_, C_ = 0x10000, 0x20000, 0x30000
+    two = lambda *v: (C.c_void_p * 2)(*v)
+    f2 = (C.c_float * 2)(1.0, -1.0)
+    cases = [
+        (h.hf_upfirdn2d_f32, (A, B_, None, 1, 4, 4, 4, 4, 1, 1, 1, 1, 0, 0, 0, 0, None), b"upfirdn2d: null pointer"),
+        (h.hf_upfirdn2d_f32, (A, B_, C_, 1, 0, 4, 4, 4, 1, 1, 1, 1, 0, 0, 0, 0, None), b"upfirdn2d: bad shape"),
+        (h.hf_upfirdn2d_f32, (A, B_, C_, 1, 4, 4, 4, 4, 1, 0, 1, 1, 0, 0, 0, 0, None), b"upfirdn2d: up/down must be"),
+        (h.hf_upfirdn2d_f32, (A, B_, C_, 1, 2, 2, 4, 4, 1, 1, 1, 1, 0, 0, 0, 0, None), b"upfirdn2d: output would be"),
+        (h.hf_bias_act_f32, (None, None, B_, 8, 0, 4, 3, 0.2, 1.0, None), b"bias_act: null pointer"),
+        (h.hf_bias_act_f32, (A, None, B_, 8, 0, 4, 2, 0.2, 1.0, None), b"bias_act: act must be 1"),
+        (h.hf_bias_act_f32, (A, None, B_, 8, 0, 0, 3, 0.2, 1.0, None), b"bias_act: bad sizes"),
+        (h.hf_bias_act_f32, (A, None, B_, 8, 2, 4, 3, 0.2, 1.0, None), b"bias_act: bias pointer is null"),
+        (h.hf_bicubic_downsample_f32, (A, None, B_, 1, 64, 64, 4, 0, None), b"bicubic_down: null pointer"),
+        (h.hf_bicubic_downsample_f32, (A, B_, C_, 1, 64, 64, 9, 0, None), b"bicubic_down: factor 9 unsupported"),
+        (h.hf_bicubic_downsample_f32, (A, B_, C_, 0, 64, 64, 4, 0, None), b"bicubic_down: bad shape"),
+        (h.hf_bicubic_downsample_f32, (A, B_, C_, 1, 6, 64, 4, 0, None), b"bicubic_down: image smaller than"),
+        (h.hf_dilate_erode_f32, (A, None, C_, None, 1, 4, 4, 1, None), b"dilate_erode: null pointer"),
+        (h.hf_dilate_erode_f32, (A, B_, C_, None, 1, 4, 4, -1, None), b"dilate_erode: bad arguments"),
+        (h.hf_dilate_erode_f32, (A, B_, C_, None, 1, 4, 4, 2, None), b"dilate_erode: workspace"),
+        (h.hf_dilate_erode_f32, (A, B_, C_, None, 50000, 200, 200, 1, None), b"dilate_erode: tensor too large"),
+        (h.hf_align_masks_f32, (A, B_, None, C_, 16, None), b"align_masks: bad arguments"),
+        (h.hf_align_masks_f32, (A, B_, C_, A, 0, None), b"align_masks: bad arguments"),
+        (h.hf_fspace_blend_f32, (A, two(B_, B_), two(C_, C_), None, f2, A, 2, 4, 8, 8, 8, 8, None),
+         b"fspace_blend: null pointer"),
+        (h.hf_fspace_blend_f32, (A, two(B_, B_), two(C_, C_), f2, None, A, 2, 4, 8, 8, 8, 8, None),
+         b"fspace_blend: null pointer"),
+        (h.hf_fspace_blend_f32, (A, two(B_, B_), two(C_, C_), f2, f2, A, 5, 4, 8, 8, 8, 8, None),
+         b"fspace_blend: 1..4 stages"),
+        (h.hf_fspace_blend_f32, (A, two(B_, B_), two(C_, C_), f2, f2, A, 2, 4, 0, 8, 8, 8, None),
+         b"fspace_blend: bad shape"),
+        (h.hf_fspace_blend_f32, (A, two(B_, None), two(C_, C_), f2, f2, A, 2, 4, 8, 8, 8, 8, None),
+         b"fspace_blend: null stage pointer"),
+    ]
+    for fn, args, msg in cases:
+        assert fn(*args) == -1, (fn.__name__, args)                   # HF_ERR_INVALID
+        assert h.hf_last_error().startswith(msg), (fn.__name__, args, h.hf_last_error())
+    assert h.hf_bias_act_f32(None, None, None, 0, 0, 1, 3, 0.2, 1.0, None) == 0          # empty input
