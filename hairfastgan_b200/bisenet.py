@@ -12,11 +12,12 @@ parameter containers.
 """
 from __future__ import annotations
 
+import functools
+
 import torch
 import torch.nn as nn
 
-from . import graphs, nn16
-from .encoders import _PackCacheMixin, _params_key
+from . import graphs, nn16, packcache
 
 __all__ = ["BiSeNet", "ConvBNReLU", "BiSeNetOutput", "AttentionRefinementModule", "ContextPath", "FeatureFusionModule",
            "Resnet18", "BasicBlock"]
@@ -173,7 +174,7 @@ class _PackedOutput:
         return nn16.bilinear_upsample_nchw(low, self.n_classes, height, width), low
 
 
-class BiSeNet(_PackCacheMixin, nn.Module):
+class BiSeNet(nn.Module):
     """model.py:217-244."""
 
     def __init__(self, n_classes, *args, **kwargs):
@@ -183,12 +184,8 @@ class BiSeNet(_PackCacheMixin, nn.Module):
         self.conv_out = BiSeNetOutput(256, 256, n_classes)
         self.conv_out16 = BiSeNetOutput(128, 64, n_classes)
         self.conv_out32 = BiSeNetOutput(128, 64, n_classes)
-        self._pk = None
 
     def _pack(self):
-        key = _params_key(self)
-        if self._pk is not None and self._pk["key"] == key:
-            return self._pk
         cp, rn = self.cp, self.cp.resnet
 
         def arm(m):
@@ -197,7 +194,7 @@ class BiSeNet(_PackCacheMixin, nn.Module):
             return {"conv": conv, "shift": shift, "w": m.conv_atten.weight, "a_scale": a_scale, "a_shift": a_shift}
 
         avg_scale, avg_shift = nn16.bn_affine(cp.conv_avg.bn)
-        pk = {"key": key, "stem": nn16.PackedStem7x7(rn.conv1.weight, rn.bn1),
+        pk = {"stem": nn16.PackedStem7x7(rn.conv1.weight, rn.bn1),
               "blocks": [[_PackedBlock(b) for b in layer] for layer in (rn.layer1, rn.layer2, rn.layer3, rn.layer4)],
               "arm16": arm(cp.arm16), "arm32": arm(cp.arm32),
               "head32": cp.conv_head32.packed(), "head16": cp.conv_head16.packed(),
@@ -205,10 +202,9 @@ class BiSeNet(_PackCacheMixin, nn.Module):
               "ffm": self.ffm.convblk.packed(),
               "out": _PackedOutput(self.conv_out), "out16": _PackedOutput(self.conv_out16),
               "out32": _PackedOutput(self.conv_out32)}
-        self._pk = pk
         return pk
 
-    def _trunk(self, x):
+    def _trunk(self, pk, x):
         """Everything up to the three head inputs (fuse, feat16_up, feat32_up) -- model.py:226-234."""
         if self.training:
             raise RuntimeError("BiSeNet: only eval-mode (running BatchNorm statistics) forward is implemented")
@@ -219,7 +215,6 @@ class BiSeNet(_PackCacheMixin, nn.Module):
         H, W = x.shape[2:]
         if H % 32 or W % 32:
             raise NotImplementedError(f"BiSeNet: input size {H}x{W} must be a multiple of 32")
-        pk = self._pack()
         # ---- Resnet18 (resnet.py:68-79)
         f = nn16.maxpool3x3s2(pk["stem"](x))
         feats = []
@@ -247,7 +242,7 @@ class BiSeNet(_PackCacheMixin, nn.Module):
         feat, _, _ = pk["ffm"][0](fcat, shift=pk["ffm"][1], act=3)
         atten = nn16.se_gate(feat, self.ffm.conv1.weight, self.ffm.conv2.weight)
         fuse, _ = nn16.scale_add(feat, atten, feat)                                                 # feat*atten + feat
-        return pk, fuse, feat16_up, feat32_up, H, W
+        return fuse, feat16_up, feat32_up, H, W
 
     def _check(self, x):
         if self.training:
@@ -258,12 +253,13 @@ class BiSeNet(_PackCacheMixin, nn.Module):
     @torch.no_grad()
     def forward(self, x, return_lowres: bool = False):
         self._check(x)
+        pk, key = packcache.get(self, "_hf_pack", (self,), nn16.default_dtype(), self._pack)
         if return_lowres:
-            return self._forward_impl(x, True)
-        return graphs.run(self, "fwd", _params_key(self), self._forward_impl, x)
+            return self._forward_impl(pk, x, True)
+        return graphs.run(self, "fwd", key, functools.partial(self._forward_impl, pk), x)
 
-    def _forward_impl(self, x, return_lowres: bool = False):
-        pk, fuse, feat16_up, feat32_up, H, W = self._trunk(x)
+    def _forward_impl(self, pk, x, return_lowres: bool = False):
+        fuse, feat16_up, feat32_up, H, W = self._trunk(pk, x)
         # ---- heads + bilinear upsampling (model.py:235-241)
         o, lo = pk["out"](fuse, H, W)
         o16, lo16 = pk["out16"](feat16_up, H, W)
@@ -279,9 +275,10 @@ class BiSeNet(_PackCacheMixin, nn.Module):
         the two auxiliary heads (training-time supervision, model.py:236-237) are not evaluated and the upsampling is
         fused with the arg-max (``hf_bilinear_argmax_nchw_f32``), so the 19 x H x W fp32 logits are never written."""
         self._check(x)
-        return graphs.run(self, "labels", _params_key(self), self._parse_impl, x)
+        pk, key = packcache.get(self, "_hf_pack", (self,), nn16.default_dtype(), self._pack)
+        return graphs.run(self, "labels", key, functools.partial(self._parse_impl, pk), x)
 
-    def _parse_impl(self, x):
-        pk, fuse, _, _, H, W = self._trunk(x)
+    def _parse_impl(self, pk, x):
+        fuse, _, _, H, W = self._trunk(pk, x)
         low = pk["out"].lowres(fuse)
         return nn16.bilinear_argmax_nchw(low, pk["out"].n_classes, H, W)

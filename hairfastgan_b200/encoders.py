@@ -17,35 +17,15 @@ Eval mode only (running statistics); CUDA only, no fallback.
 """
 from __future__ import annotations
 
+import functools
 import math
 from collections import namedtuple
 
 import torch
 from torch import nn
 
-from . import graphs, nn16
+from . import graphs, nn16, packcache
 from .model import EqualLinear
-
-
-def _params_key(module: nn.Module):
-    """Version key of every parameter / buffer (repack when a weight changes).  Walking the module tree costs
-    milliseconds for a 600-tensor encoder -- as much as its kernels at swap()'s batch sizes -- so the tensor LIST is
-    cached on the module; `nn.Module._apply` (.to / .cuda / .float: the calls that replace buffer objects) drops it
-    (`_PackCacheMixin`), `load_state_dict` copies in place and shows up in `_version`."""
-    ts = module.__dict__.get("_hf_tensors")
-    if ts is None:
-        ts = list(module.parameters()) + list(module.buffers())
-        module.__dict__["_hf_tensors"] = ts
-    return tuple([(t.data_ptr(), t._version) for t in ts])
-
-
-class _PackCacheMixin:
-    """Invalidate the cached tensor list (and with it the packed operands / captured graphs) on device / dtype moves."""
-
-    def _apply(self, fn, *args, **kwargs):
-        self.__dict__.pop("_hf_tensors", None)
-        self.__dict__.pop("_hf_graphs", None)
-        return super()._apply(fn, *args, **kwargs)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -189,7 +169,7 @@ class _PackedHeads:
         return y.reshape(b, self.n, -1)                                         # EqualLinear per head
 
 
-class Encoder4Editing(_PackCacheMixin, nn.Module):
+class Encoder4Editing(nn.Module):
     def __init__(self, num_layers, mode="ir", opts=None):
         super().__init__()
         assert num_layers in [50, 100, 152], "num_layers should be 50,100, or 152"
@@ -208,24 +188,18 @@ class Encoder4Editing(_PackCacheMixin, nn.Module):
             self.styles.append(GradualStyleBlock(512, 512, spatial))
         self.latlayer1 = nn.Conv2d(256, 512, kernel_size=1, stride=1, padding=0)
         self.latlayer2 = nn.Conv2d(128, 512, kernel_size=1, stride=1, padding=0)
-        self._pk = None
 
     def get_deltas_starting_dimensions(self):
         return list(range(self.style_count))
 
     def _pack(self):
-        key = _params_key(self)
-        if self._pk is not None and self._pk["key"] == key:
-            return self._pk
         il = self.input_layer
-        pk = {"key": key,
-              "stem": nn16.PackedStem3x3(il[0].weight, il[1], il[2].weight),      # conv + BN + PReLU, one fused kernel
+        pk = {"stem": nn16.PackedStem3x3(il[0].weight, il[1], il[2].weight),      # conv + BN + PReLU, one fused kernel
               "blocks": [m.packed() for m in self.body],
               "lat1": nn16.PackedConv2d(self.latlayer1.weight), "lat2": nn16.PackedConv2d(self.latlayer2.weight),
               "heads": [_PackedHeads(list(self.styles[:self.coarse_ind])),
                         _PackedHeads(list(self.styles[self.coarse_ind:self.middle_ind])),
                         _PackedHeads(list(self.styles[self.middle_ind:]))]}
-        self._pk = pk
         return pk
 
     @torch.no_grad()
@@ -234,10 +208,10 @@ class Encoder4Editing(_PackCacheMixin, nn.Module):
             raise RuntimeError("Encoder4Editing: only eval-mode (running BatchNorm statistics) forward is implemented")
         if not x.is_cuda:
             raise RuntimeError("Encoder4Editing: input must be a CUDA tensor (no CPU fallback)")
-        return graphs.run(self, "e4e", _params_key(self), self._forward_impl, x)
+        pk, key = packcache.get(self, "_hf_pack", (self,), nn16.default_dtype(), self._pack)
+        return graphs.run(self, "e4e", key, functools.partial(self._forward_impl, pk), x)
 
-    def _forward_impl(self, x):
-        pk = self._pack()
+    def _forward_impl(self, pk, x):
         blocks = pk["blocks"]
         raw, bn = pk["stem"](x, y16b_affine=blocks[0].pre)
         taps = {}
@@ -329,7 +303,7 @@ def _load_arcface_trunk(module, path):
     module.load_state_dict(mine, strict=False)
 
 
-class fs_encoder_v2(_PackCacheMixin, nn.Module):
+class fs_encoder_v2(nn.Module):
     def __init__(self, n_styles=18, opts=None, residual=False, use_coeff=False, resnet_layer=None, video_input=False,
                  f_maps=512, stride=(1, 1)):
         super().__init__()
@@ -353,16 +327,12 @@ class fs_encoder_v2(_PackCacheMixin, nn.Module):
         self._content_strides = [s]
         self.avg_pool = nn.AdaptiveAvgPool2d((3, 3))
         self.styles = nn.ModuleList([nn.Linear(960 * 9, 512) for _ in range(n_styles)])
-        self._pk = None
 
     def _content_branches(self):
         """[(BN, conv3x3, BN, PReLU, conv3x3(stride), BN)] -- one per content output."""
         return [self.content_layer]
 
     def _pack(self):
-        key = _params_key(self)
-        if self._pk is not None and self._pk["key"] == key:
-            return self._pk
         branches = []
         for cl, stride in zip(self._content_branches(), self._content_strides):
             c_mid_scale, c_mid_shift = nn16.bn_affine(cl[2])
@@ -372,7 +342,7 @@ class fs_encoder_v2(_PackCacheMixin, nn.Module):
                              "slope": cl[3].weight.detach().float().contiguous(),
                              "conv2": nn16.PackedConv2d(cl[4].weight, c_out_scale, stride=stride),
                              "shift2": c_out_shift})
-        pk = {"key": key, "stem": nn16.PackedStem3x3(self.conv[0].weight, self.conv[1], self.conv[2].weight),
+        pk = {"stem": nn16.PackedStem3x3(self.conv[0].weight, self.conv[1], self.conv[2].weight),
               "stages": [[b.packed() for b in blk] for blk in (self.block_1, self.block_2, self.block_3, self.block_4)],
               "content": branches,
               # the n_styles nn.Linear(960*9, 512) heads (feature_style_encoder.py:44-45,62-64) stacked: ONE 1x1
@@ -380,17 +350,15 @@ class fs_encoder_v2(_PackCacheMixin, nn.Module):
               "style": nn16.PackedConv2d(torch.cat([s.weight.detach().float() for s in self.styles], 0)[:, :, None, None]),
               "style_b": torch.cat([s.bias.detach().float() for s in self.styles], 0).contiguous(),
               "n_styles": len(self.styles)}
-        self._pk = pk
         return pk
 
-    def _trunk(self, x):
+    def _trunk(self, pk, x):
         """conv stem -> block_1..4 with the pooled features and the content branches: (latents, [content...])."""
         name = type(self).__name__
         if self.training:
             raise RuntimeError(f"{name}: only eval-mode (running BatchNorm statistics) forward is implemented")
         if not x.is_cuda:
             raise RuntimeError(f"{name}: input must be a CUDA tensor (no CPU fallback)")
-        pk = self._pack()
         blocks = [b for st in pk["stages"] for b in st]
         ends, n = [], 0
         for st in pk["stages"]:
@@ -427,4 +395,5 @@ class fs_encoder_v2(_PackCacheMixin, nn.Module):
             raise RuntimeError(f"{name}: only eval-mode (running BatchNorm statistics) forward is implemented")
         if not x.is_cuda:
             raise RuntimeError(f"{name}: input must be a CUDA tensor (no CPU fallback)")
-        return graphs.run(self, "trunk", _params_key(self), self._trunk, x)
+        pk, key = packcache.get(self, "_hf_pack", (self,), nn16.default_dtype(), self._pack)
+        return graphs.run(self, "trunk", key, functools.partial(self._trunk, pk), x)

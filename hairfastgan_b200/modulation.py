@@ -14,7 +14,7 @@ A stack is 5 ``ModulationModule(L, last=i == 4, inp, middle)``; one call of the 
 
 PostProcess's two stacks (``to_latent_1`` / ``to_latent_2``) run in the same 6 launches, plus one ``cudaMemsetAsync``
 that zeroes the chain's per-(sample, slice) completion counters.  Weights are packed by
-state-dict key and re-packed when a parameter changes; operands are 16-bit in the encoder family's type
+state-dict key and re-packed by the rule of ``packcache``; operands are 16-bit in the encoder family's type
 (``nn16.default_dtype``), accumulation and statistics fp32.  The forward draws no random numbers and never waits for
 the device.  Only HairFast's three configurations are supported: L = 6 and 18 with (inp, middle) = (512, 512), L = 12
 with (1536, 1024).
@@ -25,7 +25,7 @@ import ctypes as C
 
 import torch
 
-from . import _lib, nn16
+from . import _lib, nn16, packcache
 
 DIM = 512
 MODULES = 5
@@ -87,33 +87,10 @@ class PackedStacks:
         self.desc = _lib.hf_mod_desc(layers, inp, middle, len(stacks), dtype)
 
 
-def _stack_key(stack):
-    """Identity of every submodule and parameter in the stack's tree, and storage and version of every parameter.  The
-    reference's nn.ModuleList has no hook that would drop a cached parameter list, so the tree is read each call: a
-    replaced or added submodule (``stack[i].fc = nn.Linear(...)``) changes the key.  The cached module list keeps the
-    old objects alive, so their ids cannot be reused by new ones."""
-    mods = stack.__dict__.get("_hf_mod_tree")
-    if mods is None:
-        mods = stack.__dict__["_hf_mod_tree"] = list(stack.modules())
-    ids = [id(x) for m in mods for d in (m._modules, m._parameters) for x in d.values()]
-    if ids != stack.__dict__.get("_hf_mod_ids"):
-        mods = stack.__dict__["_hf_mod_tree"] = list(stack.modules())
-        ids = stack.__dict__["_hf_mod_ids"] = [id(x) for m in mods for d in (m._modules, m._parameters)
-                                               for x in d.values()]
-    return tuple(ids), tuple([(p.data_ptr(), p._version) for m in mods for p in m._parameters.values()
-                              if p is not None])
-
-
 def pack(owner, stacks, layers: int) -> PackedStacks:
-    """The packed stacks, cached on ``owner`` and re-packed when a parameter (in place, by .to() or by replacing a
-    submodule) or the dtype changes."""
+    """The packed stacks, cached on ``owner`` (whose class fixes ``layers``) by ``packcache``."""
     dt = nn16.default_dtype()
-    key = (tuple(_stack_key(st) for st in stacks), layers, dt)
-    pk = owner.__dict__.get("_hf_mod_pack")
-    if pk is None or pk[0] != key:
-        pk = (key, PackedStacks(stacks, layers, dt))
-        owner.__dict__["_hf_mod_pack"] = pk
-    return pk[1]
+    return packcache.get(owner, "_hf_mod_pack", stacks, dt, lambda: PackedStacks(stacks, layers, dt))[0]
 
 
 # How a [batch, layers, 512] operand is read from its tensor; each caller names the form it means.

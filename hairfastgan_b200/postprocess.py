@@ -15,12 +15,14 @@ strict=True)`` of a PostProcess checkpoint works).  CUDA tensors only, eval mode
 """
 from __future__ import annotations
 
+import functools
+
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import graphs, nn16
-from .encoders import IBasicBlock, _PackCacheMixin, _params_key, fs_encoder_v2
+from . import graphs, nn16, packcache
+from .encoders import IBasicBlock, fs_encoder_v2
 
 __all__ = ["FeatureEncoder", "FeatureEncoderMult", "FeatureiResnet", "IBasicBlock", "conv1x1", "conv3x3",
            "transform_to_256"]
@@ -86,7 +88,6 @@ class FeatureEncoderMult(FeatureEncoder):
                 nn.BatchNorm2d(512, eps=1e-05)))
             self._content_strides.append(stride[0])
         self._content_stage = 2 if max(fs_layers) <= 7 else 1      # after block_3 / after block_2 (Net.py:453-470)
-        self._pk = None
 
     def _content_branches(self):
         return list(self.content_layer)
@@ -96,7 +97,7 @@ class FeatureEncoderMult(FeatureEncoder):
         return self._graphed_trunk(transform_to_256(x))
 
 
-class FeatureiResnet(_PackCacheMixin, nn.Module):
+class FeatureiResnet(nn.Module):
     """models/Encoders.py:35-57."""
 
     def __init__(self, blocks, inplanes=1024):
@@ -110,13 +111,9 @@ class FeatureiResnet(_PackCacheMixin, nn.Module):
                 res_blocks[f"res_block_{n}_{k}"] = IBasicBlock(inplanes, planes, 1, downsample, 1, 64, 1)
                 inplanes = planes
         self.res_blocks = nn.ModuleDict(res_blocks)
-        self._pk = None
 
     def _pack(self):
-        key = _params_key(self)
-        if self._pk is None or self._pk[0] != key:
-            self._pk = (key, [m.packed() for m in self.res_blocks.values()])
-        return self._pk[1]
+        return [m.packed() for m in self.res_blocks.values()]
 
     @torch.no_grad()
     def forward(self, x):
@@ -124,10 +121,10 @@ class FeatureiResnet(_PackCacheMixin, nn.Module):
             raise RuntimeError("FeatureiResnet: only eval-mode (running BatchNorm statistics) forward is implemented")
         if not x.is_cuda:
             raise RuntimeError("FeatureiResnet: input must be a CUDA tensor (no CPU fallback)")
-        return graphs.run(self, "res", _params_key(self), self._forward_impl, x)
+        blocks, key = packcache.get(self, "_hf_pack", (self,), nn16.default_dtype(), self._pack)
+        return graphs.run(self, "res", key, functools.partial(self._forward_impl, blocks), x)
 
-    def _forward_impl(self, x):
-        blocks = self._pack()
+    def _forward_impl(self, blocks, x):
         # x is fp32 NCHW (torch.cat of the two content maps); the first block's BatchNorm rides on the layout change
         raw = nn16.to_nhwc16(x)
         bn = nn16.to_nhwc16(x, scale=blocks[0].pre[0], shift=blocks[0].pre[1])

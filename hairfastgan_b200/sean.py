@@ -33,8 +33,7 @@ from typing import List, Optional, Sequence
 
 import torch
 
-from . import _lib, nn16
-from .encoders import _params_key
+from . import _lib, nn16, packcache
 
 N_CLASSES = 19
 STYLE = 512
@@ -153,12 +152,8 @@ class PackedSEAN:
 
 
 def _pack(netG) -> PackedSEAN:
-    key = (_params_key(netG), nn16.default_dtype())
-    pk = netG.__dict__.get("_hf_sean_pack")
-    if pk is None or pk[0] != key:
-        pk = (key, PackedSEAN(netG))
-        netG.__dict__["_hf_sean_pack"] = pk
-    return pk[1]
+    dt = nn16.default_dtype()
+    return packcache.get(netG, "_hf_sean_pack", (netG,), dt, lambda: PackedSEAN(netG, dt))[0]
 
 
 def mean_style_codes(device) -> torch.Tensor:
@@ -209,12 +204,8 @@ class PackedZencoder:
 
 
 def _pack_zencoder(zenc) -> PackedZencoder:
-    key = (_params_key(zenc), nn16.default_dtype())
-    pk = zenc.__dict__.get("_hf_zencoder_pack")
-    if pk is None or pk[0] != key:
-        pk = (key, PackedZencoder(zenc))
-        zenc.__dict__["_hf_zencoder_pack"] = pk
-    return pk[1]
+    dt = nn16.default_dtype()
+    return packcache.get(zenc, "_hf_zencoder_pack", (zenc,), dt, lambda: PackedZencoder(zenc, dt))[0]
 
 
 # ------------------------------------------------------------------------------------------------ kernel wrappers

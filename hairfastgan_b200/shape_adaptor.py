@@ -21,8 +21,8 @@ Per MaskDecoder (Linear -> [2048,2,2], 7 x [nearest 2x, Conv 3x3, LayerNorm, Lea
 
 The CtrlHair LayerNorm (whole-sample mean and unbiased std, then per-channel gamma / beta) is
 ``hf_shape_layer_norm_lrelu``.  Activations are 16-bit NHWC in the encoder family's type (``nn16.default_dtype``).
-Networks are packed by state-dict key, each on its own (``get_new_shape`` never packs the encoders), and re-packed when
-a parameter's storage or version changes.
+Networks are packed by state-dict key, each on its own (``get_new_shape`` never packs the encoders), and re-packed by
+the rule of ``packcache``.
 """
 from __future__ import annotations
 
@@ -31,8 +31,7 @@ from typing import Optional
 import torch
 import torch.nn.functional as F
 
-from . import _lib, nn16
-from .encoders import _params_key
+from . import _lib, nn16, packcache
 
 N_CLASSES = 19
 HAIR_IDX = 13                  # HAIR_IDX (models/CtrlHair/global_value_utils.py:52)
@@ -162,23 +161,15 @@ class PackedDecoders:
         self.table_bias = torch.cat([self.face.out_b[:HAIR_IDX], self.hair.out_b, self.face.out_b[HAIR_IDX:]]).contiguous()
 
 
-def _cached(owner, attr: str, key, make):
-    pk = owner.__dict__.get(attr)
-    if pk is None or pk[0] != key:
-        pk = (key, make())
-        owner.__dict__[attr] = pk
-    return pk[1]
-
-
 def pack_encoder(enc, hair: bool) -> PackedEncoder:
     dt = nn16.default_dtype()
-    return _cached(enc, "_hf_shape_pack", (_params_key(enc), dt), lambda: PackedEncoder(enc, hair, dt))
+    return packcache.get(enc, "_hf_shape_pack", (enc,), dt, lambda: PackedEncoder(enc, hair, dt))[0]
 
 
 def pack_decoders(gen) -> PackedDecoders:
     dt = nn16.default_dtype()
-    key = (_params_key(gen.hair_decoder), _params_key(gen.face_decoder), dt)
-    return _cached(gen, "_hf_shape_decoders_pack", key, lambda: PackedDecoders(gen, dt))
+    return packcache.get(gen, "_hf_shape_decoders_pack", (gen.hair_decoder, gen.face_decoder), dt,
+                         lambda: PackedDecoders(gen, dt))[0]
 
 
 # ------------------------------------------------------------------------------------------------ kernel wrappers

@@ -297,6 +297,35 @@ def test_cuda_graph_replay_matches_eager(N):
     assert all(torch.equal(lab[0], o) for o in lab[1:]) and torch.equal(lab[0], seg(x[:1])[0].argmax(1))
 
 
+def test_dtype_switch_repacks_and_recaptures(N, monkeypatch):
+    """The 16-bit type is part of the pack key: after eager, captured and replayed calls in fp16, each of three bf16
+    calls (eager, capture, replay) equals a fresh module's bf16 output bit for bit."""
+    import hairfastgan_b200.encoders as E
+    import hairfastgan_b200.bisenet as B
+    from hairfastgan_b200 import graphs
+    x = (torch.rand(2, 3, 256, 256, generator=torch.Generator().manual_seed(93)) * 2 - 1).cuda()
+    flat = lambda out: [out] if torch.is_tensor(out) else list(out)            # noqa: E731
+    for make, seed in [(lambda: E.Encoder4Editing(50, "ir_se", types.SimpleNamespace(stylegan_size=1024)), 11),
+                       (lambda: E.fs_encoder_v2(n_styles=18, opts=None, stride=(2, 2)), 21),
+                       (lambda: B.BiSeNet(n_classes=19), 51)]:
+        net = make().eval()
+        net.load_state_dict(EO.synth_params_like(net, seed=seed), strict=True)
+        net = net.cuda()
+        s0 = graphs.stats()
+        monkeypatch.setenv("HAIRFAST_ENC_DTYPE", "fp16")
+        f16 = [flat(net(x)) for _ in range(3)]
+        monkeypatch.setenv("HAIRFAST_ENC_DTYPE", "bf16")
+        b16 = [flat(net(x)) for _ in range(3)]
+        s1 = graphs.stats()
+        assert s1["captures"] == s0["captures"] + 2 and s1["failed"] == s0["failed"], type(net).__name__
+        fresh = make().eval()
+        fresh.load_state_dict(net.state_dict(), strict=True)
+        ref = flat(fresh.cuda()(x))
+        assert not torch.equal(f16[2][0], ref[0]), type(net).__name__
+        for out in b16:
+            assert all(torch.equal(a, r) for a, r in zip(out, ref)), type(net).__name__
+
+
 def test_fused_stem3x3_vs_torch(N):
     """hf_stem3x3_nhwc16: Conv2d(3,64,3,1,1) + eval BatchNorm + PReLU (+ the next block's BatchNorm as second output)
     against torch fp32, on a size that is not a multiple of the 8 x 32 tile."""
